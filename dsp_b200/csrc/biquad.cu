@@ -10,6 +10,7 @@
 //   * a CTA owns two adjacent channels and a tile of 4096 frames; a lane owns one chunk of L = 16 frames of one
 //     channel (a warp = 16 consecutive chunks x 2 channels, channel fastest), the chunk's samples live in
 //     registers through all S stages;
+//   * the scan runs in a better-conditioned basis w = T^-1 z (below); z is only formed for the re-run (4);
 //   * per stage: (1) every lane needs the end state e its chunk would reach from a ZERO state; that is the
 //     dot product e = sum_i A^(L-1-i) B s_i of the chunk with a per-stage table (2 L independent FMAs instead
 //     of a serial recurrence; table built on the host in long double); (2) warp-level inclusive scan of the
@@ -18,8 +19,16 @@
 //     with A^(16 L), every lane turns the carry-in of its warp into its own start state with the binary
 //     expansion of its chunk index; (4) the lane re-runs the reference's own recurrence from that TRUE start
 //     state -- so every output sample is produced by exactly the reference's arithmetic, started from a
-//     state that differs from the sequential one only by rounding in the scan (|eig A| < 1);
+//     state that differs from the sequential one by rounding in the scan (|eig A| < 1);
 //   * longer calls loop over tiles, carrying the per-stage state through shared memory.
+// Basis: with both poles near z = 1 (low corners at high rates: 10 Hz at 192 kHz) the companion matrix A is far from
+// normal -- A^k has entries of order k that cancel to a state of order 1 -- and a scan on z loses about log2(k) bits,
+// 50 to 150 times the sequential recurrence's own error.  With alpha = -c3 / 2 (the poles' mean) and
+// eps = sqrt|alpha^2 - c4| (half their distance), T = [[1, 0], [-alpha, eps]] turns A into M = T^-1 A T =
+// [[alpha, eps], [+-eps, alpha]]: symmetric for real poles, a scaled rotation for complex ones, normal either way, so
+// the powers M^k stay bounded by 1 and the scan keeps the precision of its inputs.  eps is clamped below at 1/32 for
+// (near-)double poles, where T would be singular; M is then only mildly non-normal.  Measured on the 10 Hz / 192 kHz
+// sections the GPU lands within a few times the FP64 recurrence's error (tests/test_gpu_accuracy.py).
 // A stage that does not act on a channel carries the identity section {1,0,0,0,0}.
 // Global accesses: one load instruction of a warp touches 16 rows (frames) and uses 16 contiguous bytes of
 // each -- half of every 32-byte sector, the neighbouring CTA uses the other half at about the same time, so
@@ -32,10 +41,12 @@ namespace dspb200 {
 
 constexpr int BQ_L = 16;           // frames per lane
 constexpr int BQ_MAX_STAGES = 16;  // stages fused into one operator
-constexpr int BQ_NPOW = 6;         // A^(L 2^r), r = 0..5
-// per channel and stage: 5 coefficients (+1 pad), BQ_NPOW 2x2 matrices, and G[i] = A^(L-1-i) B (2 x L), contiguous;
-// every piece starts on a 16-byte boundary so that the kernel reads the table with 128-bit shared loads
-constexpr int BQ_OFF_P = 6, BQ_OFF_G = BQ_OFF_P + 4 * BQ_NPOW;
+constexpr int BQ_NPOW = 6;         // M^(L 2^r), r = 0..5
+// per channel and stage: 5 coefficients (+1 pad), BQ_NPOW 2x2 matrices M^(L 2^r), the basis T and T^-1 (2x2 each), and
+// G[i] = T^-1 A^(L-1-i) B (2 x L), contiguous; every piece starts on a 16-byte boundary so that the kernel reads the
+// table with 128-bit shared loads
+constexpr double BQ_EPS_MIN = 1.0 / 32;
+constexpr int BQ_OFF_P = 6, BQ_OFF_T = BQ_OFF_P + 4 * BQ_NPOW, BQ_OFF_G = BQ_OFF_T + 8;
 constexpr int BQ_TBL = BQ_OFF_G + 2 * BQ_L;
 static_assert(BQ_TBL % 2 == 0 && BQ_OFF_G % 2 == 0, "table pieces must stay 16-byte aligned");
 
@@ -156,8 +167,9 @@ __global__ void __launch_bounds__(BqCfg<CH, SPLIT>::THREADS, SPLIT ? 2 : 1) k_bq
 				carry[st][ch] = make_double2(__ldcg(&sp.xstate[o * 2]), __ldcg(&sp.xstate[o * 2 + 1]));
 			}
 			__syncthreads();
-			// (3) carry into this warp, then into this lane
-			double2 cin = carry[st][ch];
+			// (3) carry into this warp, then into this lane (the carried state is a true z: into the scan's basis)
+			const double2 tb0 = t[BQ_OFF_T / 2], tb1 = t[BQ_OFF_T / 2 + 1], ti0 = t[BQ_OFF_T / 2 + 2], ti1 = t[BQ_OFF_T / 2 + 3];
+			double2 cin = m2_apply(M2{ ti0.x, ti0.y, ti1.x, ti1.y }, carry[st][ch]);
 			for (int k = 0; k < w; ++k) {
 				const double2 u = m2_apply(P[LOGW], cin);
 				cin = make_double2(u.x + tot[k][ch].x, u.y + tot[k][ch].y);
@@ -165,7 +177,8 @@ __global__ void __launch_bounds__(BqCfg<CH, SPLIT>::THREADS, SPLIT ? 2 : 1) k_bq
 #pragma unroll
 			for (int r = 0; r < LOGW; ++r)
 				if ((jl >> r) & 1) cin = m2_apply(P[r], cin);
-			double m0 = z.x + cin.x, m1 = z.y + cin.y;
+			const double2 zs = m2_apply(M2{ tb0.x, tb0.y, tb1.x, tb1.y }, make_double2(z.x + cin.x, z.y + cin.y));
+			double m0 = zs.x, m1 = zs.y;
 			// (4) the real run from the true start state
 #pragma unroll
 			for (int i = 0; i < BQ_L; ++i) {
@@ -292,9 +305,21 @@ Op *make_biquad_op(int slab_channels, int fs, int n_stages, const double *coefs)
 			double *t = &tbl[((size_t) c * S + st) * BQ_TBL];
 			for (int k = 0; k < 5; ++k) t[k] = cf[k];
 			// A = [[-c3, 1], [-c4, 0]], B = (c1 - c3 c0, c2 - c4 c0): z' = A z + B s   (biquad.h:79-81 with r = c0 s + m0)
-			const long double A[4] = { -(long double) cf[3], 1.0L, -(long double) cf[4], 0.0L };
-			const long double Bv[2] = { (long double) cf[1] - (long double) cf[3] * cf[0], (long double) cf[2] - (long double) cf[4] * cf[0] };
-			// G[i] = A^(L-1-i) B, i = L-1 .. 0, and A^L on the way
+			const long double Az[4] = { -(long double) cf[3], 1.0L, -(long double) cf[4], 0.0L };
+			const long double Bz[2] = { (long double) cf[1] - (long double) cf[3] * cf[0], (long double) cf[2] - (long double) cf[4] * cf[0] };
+			// the scan's basis (header): z = T w, w' = M w + T^-1 B s
+			const long double al = -(long double) cf[3] / 2, d2 = al * al - (long double) cf[4];
+			long double eps = sqrtl(fabsl(d2));
+			if (eps < BQ_EPS_MIN) eps = BQ_EPS_MIN;
+			const long double T[4] = { 1.0L, 0.0L, -al, eps }, Ti[4] = { 1.0L, 0.0L, al / eps, 1.0L / eps };
+			const long double AT[4] = { Az[0] * T[0] + Az[1] * T[2], Az[0] * T[1] + Az[1] * T[3], Az[2] * T[0] + Az[3] * T[2], Az[2] * T[1] + Az[3] * T[3] };
+			const long double A[4] = { Ti[0] * AT[0] + Ti[1] * AT[2], Ti[0] * AT[1] + Ti[1] * AT[3], Ti[2] * AT[0] + Ti[3] * AT[2], Ti[2] * AT[1] + Ti[3] * AT[3] };
+			const long double Bv[2] = { Ti[0] * Bz[0] + Ti[1] * Bz[1], Ti[2] * Bz[0] + Ti[3] * Bz[1] };
+			for (int k = 0; k < 4; ++k) {
+				t[BQ_OFF_T + k] = (double) T[k];
+				t[BQ_OFF_T + 4 + k] = (double) Ti[k];
+			}
+			// G[i] = M^(L-1-i) T^-1 B, i = L-1 .. 0, and M^L on the way
 			long double g[2] = { Bv[0], Bv[1] };
 			for (int i = BQ_L - 1; i >= 0; --i) {
 				t[BQ_OFF_G + 2 * i] = (double) g[0];
@@ -307,7 +332,7 @@ Op *make_biquad_op(int slab_channels, int fs, int n_stages, const double *coefs)
 				const long double u[4] = { A[0] * a[0] + A[1] * a[2], A[0] * a[1] + A[1] * a[3], A[2] * a[0] + A[3] * a[2], A[2] * a[1] + A[3] * a[3] };
 				for (int k = 0; k < 4; ++k) a[k] = u[k];
 			}
-			// A^(L 2^r) by repeated squaring
+			// M^(L 2^r) by repeated squaring
 			for (int r = 0; r < BQ_NPOW; ++r) {
 				for (int k = 0; k < 4; ++k) t[BQ_OFF_P + 4 * r + k] = (double) a[k];
 				const long double u[4] = { a[0] * a[0] + a[1] * a[2], a[0] * a[1] + a[1] * a[3], a[2] * a[0] + a[3] * a[2], a[2] * a[1] + a[3] * a[3] };

@@ -4,10 +4,14 @@ BASELINE.json's full sizes (impulse -> IR, linearity)."""
 import numpy as np
 import pytest
 
+from accuracy import biquad_within_ref, nerr
 from conftest import rms
 
 pytestmark = pytest.mark.gpu
-RMS_TOL = 1e-10
+# errors relative to rms(want): chains and the resample operator against the FP64 oracle, and FIR alone.  Biquad
+# cascades alone are held to accuracy.biquad_within_ref; chains with a biquad AND other operators compare with the
+# FP64 oracle, whose own recurrence is up to ~3e-13 off on the 31.25 Hz eq section (biquad_within_ref's err_ref64).
+TOL, FIR_TOL, BQ_TOL = 1e-13, 1e-14, 1e-12
 
 
 def eq_coefs(gpu_lib, fs, n_stages):
@@ -24,20 +28,18 @@ def test_biquad_c2_cascade(gpu_lib):
     x = restate.sgen_sine(fs, C, 3 * F, 20.0, 20000.0) * 0.25
     t = np.arange(3 * F)[:, None] / fs
     x += 0.25 * np.sin(2 * np.pi * (100.0 + np.arange(C)[None, :]) * t)
-    want = restate.biquad_cascade(x, coefs)
     ch = gpu_lib.Chain(fs, C).add_biquad(coefs)
     got = np.concatenate([ch.run(x[i:i + F]).copy() for i in range(0, 3 * F, F)])
-    assert rms(got - want) <= RMS_TOL, rms(got - want)
+    biquad_within_ref(got, x, coefs)
     # ragged calls, same stream
     ch.reset()
     cuts = [0, 1, 33, 100, 4196, 4197, 9000, 3 * F]
     got2 = np.concatenate([ch.run(x[a:b]).copy() for a, b in zip(cuts[:-1], cuts[1:])])
-    assert rms(got2 - want) <= RMS_TOL
+    biquad_within_ref(got2, x, coefs)
     ch.close()
 
 
 def test_biquad_per_channel_coefficients_and_long_cascade(gpu_lib):
-    from oracle import restate
     fs, C, S = 44100, 7, 20      # 20 stages -> two fused operators of <= 16
     rng = np.random.default_rng(3)
     coefs = np.zeros((S, C, 5))
@@ -46,11 +48,10 @@ def test_biquad_per_channel_coefficients_and_long_cascade(gpu_lib):
             coefs[s, c] = gpu_lib.biquad_design(13, fs, 40.0 * (1.3 ** s) + 3 * c, 0.7 + 0.1 * c, rng.uniform(-6, 6))
     coefs[3, 2] = [1, 0, 0, 0, 0]
     x = rng.standard_normal((5000, C)) * 0.1
-    want = restate.biquad_cascade(x, coefs)
     ch = gpu_lib.Chain(fs, C).add_biquad(coefs)
     assert ch.n_ops == 2
     got = np.concatenate([ch.run(x[i:i + 999]).copy() for i in range(0, 5000, 999)])
-    assert rms(got - want) <= RMS_TOL
+    biquad_within_ref(got, x, coefs)
     ch.close()
 
 
@@ -66,7 +67,7 @@ def test_fir_p_block_sizes(gpu_lib, block):
     want = restate.fir_stream(x, h, selector=sel)
     ch = gpu_lib.Chain(fs, C).add_fir(h, selector=sel)
     got = np.concatenate([ch.run(x[i:i + block]).copy() for i in range(0, N, block)])
-    assert rms(got - want) <= RMS_TOL, rms(got - want)
+    assert nerr(got, want)[0] <= FIR_TOL, rms(got - want)
     assert np.array_equal(got[:, 2], x[:, 2]) and np.array_equal(got[:, 4], x[:, 4])
     ch.close()
 
@@ -83,7 +84,7 @@ def test_fir_p_ragged_calls_and_partition_hint(gpu_lib):
         ch = gpu_lib.Chain(fs, C).add_fir(h, block_hint=hint)
         cuts = sorted(set([0, N] + list(rng.integers(1, N, 25))))
         got = np.concatenate([ch.run(x[a:b]).copy() for a, b in zip(cuts[:-1], cuts[1:])])
-        assert rms(got - want) <= RMS_TOL, (hint, rms(got - want))
+        assert nerr(got, want)[0] <= FIR_TOL, (hint, rms(got - want))
         ch.close()
 
 
@@ -99,28 +100,43 @@ def test_fir_latency_ring(gpu_lib):
     for block in (100, 512, 3000):
         ch = gpu_lib.Chain(fs, C).add_fir(h, latency=L)
         got = np.concatenate([ch.run(x[i:i + block]).copy() for i in range(0, 9000, block)])
-        assert rms(got - want) <= RMS_TOL, block
+        assert nerr(got, want)[0] <= FIR_TOL, block
         ch.close()
 
 
-@pytest.mark.parametrize("rates", [(44100, 48000), (48000, 44100), (48000, 96000), (96000, 48000), (44100, 32000)])
+RATIOS = [(44100, 48000), (48000, 44100), (48000, 96000), (96000, 48000), (44100, 32000), (44100, 96000), (44100, 192000),
+          (192000, 44100), (96000, 44100), (88200, 44100), (44100, 88200), (48000, 8000), (8000, 48000), (11025, 48000),
+          (8000, 44100)]
+
+
+@pytest.mark.parametrize("rates", RATIOS)
 def test_resample_ratios(gpu_lib, have_ref, rates):
+    """Large n (44100 -> 192000 is 640/147), sinc_os = 1 (2:1 and 1:2), 1:6 and 6:1 (len_mult > 16, rounded up by
+    next_fast_fftw_len), on 3 and 2 channels (FMA kernel, single channels and pairs) and 4 (tensor-core kernel); drain
+    included, per-call frame counts identical, RMS error <= 1e-13 of rms(want).  Measured against the compiled reference
+    (H100 80GB HBM3, 400 W): worst 2.7e-15 over the ratios and channel counts."""
     from oracle import restate
     fi, fo = rates
-    C = 5
+    r = restate.Resampler(fi, fo, 1)
+    p = gpu_lib.resample_params(fi, fo)
+    assert (p["n"], p["d"], p["in_len"], p["out_len"], p["out_delay"]) == (r.n, r.d, r.in_len, r.out_len, r.out_delay)
+    if rates in ((48000, 8000), (8000, 48000), (88200, 44100), (44100, 88200)):
+        raw = (r.m + 1 + max(r.n, r.d) - 1) // max(r.n, r.d)
+        assert raw > 16 and r.in_len // r.d == restate.next_fast_fftw_len(raw) != raw, (raw, r.in_len // r.d)
     rng = np.random.default_rng(fi + fo)
-    x = rng.standard_normal((9000, C)) * 0.3
+    x = rng.standard_normal((9000, 4)) * 0.3
     x[:, 0] = np.sin(2 * np.pi * 1000.0 * np.arange(9000) / fi)
     if have_ref:
         from oracle import ref
-        want, wcounts = ref.RefChain("resample %d" % fo, fi, C).process(x, 1024)
+        want, wcounts = ref.RefChain("resample %d" % fo, fi, 4).process(x, 1024)
     else:
-        want, wcounts = restate.Resampler(fi, fo, C).process(x, 1024)
-    ch = gpu_lib.Chain(fi, C).add_resample(fo)
-    got, counts = ch.process(x, 1024)
-    assert counts == list(wcounts)
-    assert rms(got - want) <= RMS_TOL, rms(got - want)
-    ch.close()
+        want, wcounts = restate.Resampler(fi, fo, 4).process(x, 1024)
+    for C in (3, 2, 4):
+        ch = gpu_lib.Chain(fi, C).add_resample(fo)
+        got, counts = ch.process(x[:, :C], 1024)
+        ch.close()
+        assert counts == list(wcounts), C
+        assert nerr(got, want[:, :C])[0] <= TOL, (C, nerr(got, want[:, :C]))
 
 
 @pytest.mark.parametrize("channels", [1, 2, 4, 6, 36, 132])
@@ -139,15 +155,14 @@ def test_resample_channel_counts_pick_every_kernel_variant(gpu_lib, have_ref, ch
     else:
         r = restate.Resampler(fi, fo, channels)
     ch = gpu_lib.Chain(fi, channels).add_resample(fo)
-    pos = 0
+    pos, gots, wants = 0, [], []
     for n in sizes:
         blk = x[pos:pos + n]
         pos += n
-        want = r.run(blk)
-        got = ch.run(blk).copy()
-        assert got.shape == want.shape
-        if want.size:
-            assert rms(got - want) <= RMS_TOL
+        wants.append(r.run(blk))
+        gots.append(ch.run(blk).copy())
+        assert gots[-1].shape == wants[-1].shape
+    assert nerr(np.concatenate(gots), np.concatenate(wants))[0] <= TOL
     ch.close()
 
 
@@ -191,7 +206,7 @@ def test_full_size_linearity_property(gpu_lib):
     assert rms(y12 - (0.5 * y1 - 2.0 * y2)) <= 1e-13
     # and one channel against the oracle's plain convolution
     want = restate.fir_stream(x1[:, 17:18], h)
-    assert rms(y1[:, 17:18] - want) <= RMS_TOL
+    assert nerr(y1[:, 17:18], want)[0] <= FIR_TOL
 
 
 def test_device_resident_mode(gpu_lib):
@@ -293,7 +308,7 @@ def test_fir_p_large_and_odd_blocks(gpu_lib, block, taps):
     got = np.concatenate([ch.run(x[i:i + block]).copy() for i in range(0, N, block)])
     plan = ch.describe()[0]
     assert plan["planned"] == 1
-    assert rms(got - want) <= RMS_TOL, (plan, rms(got - want))
+    assert nerr(got, want)[0] <= FIR_TOL, (plan, rms(got - want))
     ch.close()
 
 
@@ -315,10 +330,10 @@ def test_fir_p_bulk_form_mixes_with_ragged_calls(gpu_lib, shared):
         outs.append(ch.run(x[pos:pos + n]).copy())
         pos += n
     got = np.concatenate(outs)
-    assert rms(got - want) <= RMS_TOL, rms(got - want)
+    assert nerr(got, want)[0] <= FIR_TOL, rms(got - want)
     ch.reset()
     got2 = np.concatenate([ch.run(x[i:i + 32768]).copy() for i in range(0, 3 * 32768, 32768)])
-    assert rms(got2 - want[:3 * 32768]) <= RMS_TOL
+    assert nerr(got2, want[:3 * 32768])[0] <= FIR_TOL
     ch.close()
 
 
@@ -341,11 +356,11 @@ def test_fir_p_single_level_with_tail(gpu_lib, block, taps, shared):
     assert len(plan["levels"]) == 1 and plan["tail_pf"] == 2, plan
     assert (plan["t_batch"] > 0) == (plan["levels"][0]["P"] >= 11), plan
     got = np.concatenate([ch.run(x[i:i + block]).copy() for i in range(0, N, block)])
-    assert rms(got - want) <= RMS_TOL, (plan, rms(got - want))
+    assert nerr(got, want)[0] <= FIR_TOL, (plan, rms(got - want))
     ch.reset()
     cuts = sorted(set([0, N, 3 * block, 4 * block, 5 * block, 9 * block] + list(rng.integers(1, N, 12))))
     got2 = np.concatenate([ch.run(x[a:b]).copy() for a, b in zip(cuts[:-1], cuts[1:])])
-    assert rms(got2 - want) <= RMS_TOL, (plan, rms(got2 - want))
+    assert nerr(got2, want)[0] <= FIR_TOL, (plan, rms(got2 - want))
     ch.close()
 
 
@@ -377,7 +392,7 @@ def test_fir_direct_block_io_variants(gpu_lib, case):
     ch.add_fir(h, selector=sel, latency=lat, block_hint=F)
     want = restate.fir_stream(xin, h, selector=sel, latency=lat)
     got = np.concatenate([ch.run(x[i:i + F]).copy() for i in range(0, x.shape[0], F)])
-    assert rms(got - want) <= RMS_TOL, (case, rms(got - want))
+    assert nerr(got, want)[0] <= (BQ_TOL if case == "biquad_first" else FIR_TOL), (case, rms(got - want))
     ch.close()
 
 
@@ -391,10 +406,9 @@ def test_full_size_config2_biquad_cascade(gpu_lib):
     t = np.arange(nblk * F)[:, None] / fs
     x += 0.25 * np.sin(2 * np.pi * (100.0 + np.arange(C)[None, :]) * t)
     g = 10.0 ** (-12.0 / 20.0)
-    want = restate.biquad_cascade(x * g, coefs)
     ch = gpu_lib.Chain(fs, C).add_gain(np.full(C, g)).add_biquad(coefs)
     got = np.concatenate([ch.run(x[i:i + F]).copy() for i in range(0, nblk * F, F)])
-    assert rms(got - want) <= RMS_TOL, rms(got - want)
+    biquad_within_ref(got, x * g, coefs)
     ch.close()
 
 
@@ -417,7 +431,7 @@ def test_full_size_config4_resample(gpu_lib, have_ref):
         want = r.run(base[i:i + F])
         got = ch.run(x[i:i + F]).copy()
         assert got.shape == (want.shape[0], C)
-        assert rms(got[:, :8] - want) <= RMS_TOL
+        assert nerr(got[:, :8], want)[0] <= TOL
         assert np.array_equal(got, np.tile(got[:, :8], (1, C // 8)))
     ch.close()
 
@@ -439,7 +453,7 @@ def test_full_size_config5_chain_share(gpu_lib, have_ref):
         want = r.run(y[i:i + F])
         got = ch.run(x[i:i + F]).copy()
         assert got.shape == (want.shape[0], C)
-        assert rms(got[:, :4] - want) <= RMS_TOL
+        assert nerr(got[:, :4], want)[0] <= BQ_TOL
         assert np.array_equal(got, np.tile(got[:, :4], (1, C // 4)))
     ch.close()
 
@@ -489,5 +503,5 @@ def test_fir_replans_after_unrepresentative_first_call(gpu_lib):
         if i == 1:
             assert ch.describe()[0]["levels"][0]["B"] == 2048, ch.describe()[0]
     got = np.concatenate(outs)
-    assert rms(got - want) <= RMS_TOL, rms(got - want)
+    assert nerr(got, want)[0] <= FIR_TOL, rms(got - want)
     ch.close()
