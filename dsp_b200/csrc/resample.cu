@@ -525,8 +525,24 @@ struct ResampleOp : Op {
 	int in_buf_pos = 0, out_buf_pos = 0, has_output = 0;
 	int is_draining = 0;
 	long drain_pos = 0, drain_frames = 0;
+	// DSP_B200_RS_TILE, read when the operator is made: 0 auto, 1..3 the FMA tiles (16x4, 16x2, 8x1), 4 tensor-core
+	// kernel, 5..7 the same with the tap tile double-buffered (cp.async) and the input rows requested 2 / 3 / 2 steps
+	// ahead at 4 / 3 / 3 CTAs per SM.  A forced tile the channel count cannot use falls back to the default.
+	int force_tile = 0;
+	// the last launch, for describe(): kernel, tile, warps per CTA, input-row steps requested ahead (0: FMA kernel)
+	const char *last_kernel = "";
+	int last_tile = 0, last_warps = 0, last_depth = 0;
 
 	const char *name() const override { return "resample"; }
+
+	std::string describe() const override
+	{
+		char buf[384];
+		snprintf(buf, sizeof(buf), "{\"op\":\"resample\",\"n\":%d,\"d\":%d,\"in_len\":%d,\"out_len\":%d,\"out_delay\":%d,\"ring_len\":%ld,"
+		         "\"force_tile\":%d,\"kernel\":\"%s\",\"tile\":%d,\"warps\":%d,\"depth\":%d}",
+		         p.n, p.d, p.in_len, p.out_len, p.out_delay, ring_len, force_tile, last_kernel, last_tile, last_warps, last_depth);
+		return buf;
+	}
 	~ResampleOp() override { dev_free(d_G); dev_free(d_ring); }
 
 	long max_out_frames(long in_frames) const override
@@ -608,13 +624,12 @@ struct ResampleOp : Op {
 		const long first_m = emit_pos;   // emission is one contiguous raw range per call
 		if (oframes > 0) {
 			ProfScope prof("resample", st);
-			// DSP_B200_RS_TILE: 0 auto, 1..3 the FMA tiles (16x4, 16x2, 8x1), 4 tensor-core kernel, 5..7 the same with the
-			// tap tile double-buffered (cp.async) and the input rows requested 2 / 3 / 2 steps ahead at 4 / 3 / 3 CTAs per SM
-			static const int force = getenv("DSP_B200_RS_TILE") ? atoi(getenv("DSP_B200_RS_TILE")) : 0;
+			const int force = force_tile;   // 1..7 where the channel count allows it (see force_tile)
 			int tile = (C % 4 == 0) ? RS_DEFAULT_MMA : (C % 2 == 0) ? 2 : 3;
 			if (force >= 1 && force <= 7 && !(((force == 1 || force >= 4) && C % 4) || (force == 2 && C % 2))) tile = force;
 			const long sms = sm_count();   // the tensor-core kernels: warps per CTA as long as every SM still gets a few CTAs
 			if (sms < 1) return -1;
+			last_tile = tile;
 			if (tile >= 5) {
 				const long tiles = ceil_div(oframes, RSM_Q);
 				const int w = (C >= 128 && tiles * ceil_div(C, 128) >= sms * 3) ? 4 : (C >= 64 && tiles * ceil_div(C, 64) >= sms * 2) ? 2 : 1;
@@ -626,6 +641,9 @@ struct ResampleOp : Op {
 				else if (w == 2) RS_MMA2(2, 1, 2);
 				else RS_MMA2(1, 1, 2);
 #undef RS_MMA2
+				last_kernel = "k_rs_mma2";
+				last_warps = w;
+				last_depth = (w == 4 && tile == 6) ? 3 : 2;
 			}
 			else if (tile == 4) {
 				// 4 warps (128 channels) per CTA when that still gives every SM a few CTAs, else 2 or 1
@@ -635,10 +653,18 @@ struct ResampleOp : Op {
 				if (w == 4) LAUNCH((k_rs_mma<4>), grid, 128, 0, st, d_ring, ring_len, C, d_G, g_stride, g_pad, p.n, p.d, p.in_len, first_m, oframes, out);
 				else if (w == 2) LAUNCH((k_rs_mma<2>), grid, 64, 0, st, d_ring, ring_len, C, d_G, g_stride, g_pad, p.n, p.d, p.in_len, first_m, oframes, out);
 				else LAUNCH((k_rs_mma<1>), grid, 32, 0, st, d_ring, ring_len, C, d_G, g_stride, g_pad, p.n, p.d, p.in_len, first_m, oframes, out);
+				last_kernel = "k_rs_mma";
+				last_warps = w;
+				last_depth = 1;
 			}
-			else if (tile == 1) rs_launch<16, 4, 4, 2>(st, d_ring, ring_len, C, d_G, g_stride, g_pad, p, first_m, oframes, out);
-			else if (tile == 2) rs_launch<16, 2, 2, 6>(st, d_ring, ring_len, C, d_G, g_stride, g_pad, p, first_m, oframes, out);
-			else rs_launch<8, 1, 4, 4>(st, d_ring, ring_len, C, d_G, g_stride, g_pad, p, first_m, oframes, out);
+			else {
+				if (tile == 1) rs_launch<16, 4, 4, 2>(st, d_ring, ring_len, C, d_G, g_stride, g_pad, p, first_m, oframes, out);
+				else if (tile == 2) rs_launch<16, 2, 2, 6>(st, d_ring, ring_len, C, d_G, g_stride, g_pad, p, first_m, oframes, out);
+				else rs_launch<8, 1, 4, 4>(st, d_ring, ring_len, C, d_G, g_stride, g_pad, p, first_m, oframes, out);
+				last_kernel = "k_rs_poly";
+				last_warps = (tile == 2) ? 2 : 4;
+				last_depth = 0;
+			}
 			emit_pos += oframes;
 		}
 		return oframes;
@@ -673,6 +699,7 @@ Op *make_resample_op(int slab_channels, int fs_in, int fs_out, double bandwidth,
 	op->fs_in = fs_in;
 	op->fs_out = fs_out;
 	op->inplace_ok = false;
+	op->force_tile = getenv("DSP_B200_RS_TILE") ? atoi(getenv("DSP_B200_RS_TILE")) : 0;
 	if (resample_params(fs_in, fs_out, bandwidth, &op->p)) return nullptr;
 	const ResampleParams &p = op->p;
 

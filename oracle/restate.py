@@ -173,6 +173,7 @@ class Resampler:
             xx = (i * 2 - m_os) / 2.0
             s = fc_os if abs(xx) < 1e-9 else math.sin(math.pi * fc_os * xx) / (math.pi * xx)
             sinc[i] = s * _window(i / m_os)
+        self.sinc = sinc                    # kept for the extended-precision tap table (tests/accuracy.py)
         self.sinc_fr = np.fft.rfft(sinc)
         self.m = m
         self.C = channels
@@ -239,6 +240,12 @@ class Resampler:
                     self.out_buf_pos = self.out_delay
                     self.has_output = 1
         return out[:o]
+
+    def reset(self):
+        """resample.c:154-161: the drain counters are left alone."""
+        self.in_buf_pos = self.out_buf_pos = 0
+        self.has_output = 0
+        self.overlap[:] = 0.0
 
     def drain2(self, frames):
         if not self.has_output and self.in_buf_pos == 0:

@@ -2,7 +2,8 @@
 import numpy as np
 import pytest
 
-from accuracy import X_SHIFT, biquad_err, biquad_truth, dyadic_signal, dyadic_taps, exact_conv, nerr
+from accuracy import (RS_RATIOS, X_SHIFT, RsPacing, biquad_err, biquad_truth, dyadic_signal, dyadic_taps, exact_conv, nerr,
+                      resample_taps_truth, resample_truth, rs_counts, rs_nerr, taps_from_sinc)
 
 
 def _int_conv(kx, kh):
@@ -113,3 +114,142 @@ def test_long_double_truth_is_closer_to_50_digit_arithmetic():
     assert e_ld <= e_64
     assert e_ld < 1e-15 * float(np.max(np.abs(f64)))
     assert biquad_err(f64, ld) > 0.0
+
+
+# ------------------------------------------------------------------------------------------------------------
+# Resample
+# ------------------------------------------------------------------------------------------------------------
+def _ld_to_mp(a):
+    """A long double as an mpmath number (its two double parts)."""
+    import mpmath
+    hi = float(a)
+    return mpmath.mpf(hi) + mpmath.mpf(float(a - np.longdouble(hi)))
+
+
+def _mp_taps(sinc, n, in_len, entries, dps=40):
+    """G[ph][t] at the (ph, t) in `entries` by the cosine sum of resample.cu's header, in `dps`-digit arithmetic:
+    S = DFT_2K(sinc), g(tau) = 1/(2 in_len) [S_0 + 2 sum_{k<K} Re(S_k e^{i th k tau}) + Re(S_K e^{i th K tau})]."""
+    import mpmath
+    mpmath.mp.dps = dps
+    K = len(sinc) // 2
+    cs = [mpmath.cospi(mpmath.mpf(j) / K) for j in range(2 * K)]
+    sn = [mpmath.sinpi(mpmath.mpf(j) / K) for j in range(2 * K)]
+    nz = [(i, mpmath.mpf(float(v))) for i, v in enumerate(sinc) if v != 0.0]
+    S = [(mpmath.fsum(v * cs[(i * k) % (2 * K)] for i, v in nz), -mpmath.fsum(v * sn[(i * k) % (2 * K)] for i, v in nz))
+         for k in range(K + 1)]
+    Pd = 2 * in_len * n
+    out = []
+    for ph, t in entries:
+        tau = ph + t * n
+        acc = mpmath.mpf(0)
+        for k in range(1, K + 1):
+            a = mpmath.mpf(2 * ((k * tau) % Pd)) / Pd
+            term = S[k][0] * mpmath.cospi(a) - S[k][1] * mpmath.sinpi(a)
+            acc += term / 2 if k == K else term
+        out.append((S[0][0] + 2 * acc) / (2 * in_len))
+    return out
+
+
+@pytest.mark.parametrize("fs_in,fs_out", [(32000, 48000), (48000, 32000)])
+def test_resample_taps_truth_matches_40_digit_cosine_sum(fs_in, fs_out):
+    """The long-double tap table against the cosine sum in 40 digits at 50 seeded entries (3:2 and 2:3 at
+    bandwidth 0.7, where K is small): the 1 / (2 in_len) scale and the phase / tap indexing."""
+    from oracle import restate
+    r = restate.Resampler(fs_in, fs_out, 1, bw=0.7)
+    G = resample_taps_truth(fs_in, fs_out, 0.7)
+    assert G.shape == (r.n, r.in_len)
+    rng = np.random.default_rng(fs_in)
+    entries = [(int(rng.integers(r.n)), int(rng.integers(r.in_len))) for _ in range(50)]
+    want = _mp_taps(r.sinc, r.n, r.in_len, entries)
+    peak = float(np.max(np.abs(G)))
+    err = max(abs(_ld_to_mp(G[ph, t]) - w) for (ph, t), w in zip(entries, want))
+    assert err <= 1e-17 * peak, err / peak
+
+
+@pytest.mark.parametrize("K,n,in_len", [(12, 3, 8), (10, 1, 10), (10, 2, 5)])
+def test_taps_from_sinc_weights_the_last_bin_as_the_cosine_sum(K, n, in_len):
+    """A random 2K-point 'sinc' makes S_K as large as the other bins (a designed lowpass leaves it near 1e-20 of
+    ||G||, too small to see): the last bin's weight, with K below the Nyquist bin Pd / 2 and (10, 1, 10; 10, 2, 5)
+    equal to it, and the whole table, against 40 digits."""
+    rng = np.random.default_rng(K + n)
+    sinc = rng.standard_normal(2 * K)
+    G = taps_from_sinc(sinc, n, in_len)
+    entries = [(ph, t) for ph in range(n) for t in range(in_len)]
+    want = _mp_taps(sinc, n, in_len, entries)
+    err = max(abs(_ld_to_mp(G[ph, t]) - w) for (ph, t), w in zip(entries, want))
+    assert err <= 1e-17 * float(np.max(np.abs(G))), err
+
+
+def _ragged(rng, N, in_len):
+    """Cut points of a ragged stream: 1, 7, in_len - 1, in_len, in_len + 1 frames and random sizes."""
+    sizes = [1, 7, in_len - 1, in_len, in_len + 1]
+    while sum(sizes) < N:
+        sizes.append(int(rng.integers(1, 2 * in_len)))
+    cuts = np.cumsum([0] + sizes)
+    return [int(c) for c in cuts[cuts < N]] + [N]
+
+
+@pytest.mark.parametrize("bw", [0.7, 0.939, 0.99])
+@pytest.mark.parametrize("rates", RS_RATIOS)
+def test_resample_truth_matches_the_fp64_reference(have_ref, rates, bw):
+    """The LPTV sum from the long-double table, against the reference algorithm in FP64 (restate.Resampler, and the
+    compiled reference where it is built) on ragged calls with the drain: ties the formula, out_delay and the drain
+    to the reference's block-FFT form (outputs past 3000 sampled).  Bound: normalized RMS <= 2e-15 (the FP64 reference is ~4e-16 from the truth);
+    every per-call count as rs_counts replays it."""
+    from oracle import restate
+    fi, fo = rates
+    r = restate.Resampler(fi, fo, 2, bw=bw)
+    rng = np.random.default_rng(fi + fo + int(1000 * bw))
+    N = 2 * r.in_len + 300
+    x = dyadic_signal(rng, N, 2)
+    x[:, 1] = 0.9 * np.sin(2 * np.pi * 0.3 * min(fi, fo) * np.arange(N) / fi)
+    cuts = _ragged(rng, N, r.in_len)
+    block = 997
+    refs = [r]
+    if have_ref:
+        from oracle import ref
+        refs.append(ref.RefChain("resample %s %d" % (bw, fo), fi, 2))
+    G = resample_taps_truth(fi, fo, bw)
+    counts, drains = rs_counts(fi, fo, np.diff(cuts), block, bw)
+    for rr in refs:
+        outs = [rr.run(x[a:b]) for a, b in zip(cuts[:-1], cuts[1:])]
+        assert [o.shape[0] for o in outs] == counts
+        if rr is r:
+            while (y := r.drain2(block)) is not None:
+                outs.append(y)
+        else:
+            outs += rr.drain(block)
+        assert [o.shape[0] for o in outs[len(counts):]] == drains
+        got = np.concatenate(outs)
+        # every output of short streams; of long ones (large n or bandwidth) the first and last 200 and a seeded sample
+        rows = np.arange(got.shape[0])
+        if rows.size > 3000:
+            rows = np.unique(np.concatenate([rows[:200], rows[-200:], rng.choice(rows, 2600, replace=False)]))
+        want = resample_truth(x, fi, fo, bw, got.shape[0], rows=rows, G=G)
+        e = rs_nerr(got[rows], want, x, G)
+        assert e[0] <= 2e-15, (rr, e)
+
+
+@pytest.mark.parametrize("rates,bw", [((44100, 48000), 0.939), ((48000, 8000), 0.7), ((8000, 44100), 0.99)])
+def test_rs_pacing_matches_the_reference_counts(rates, bw):
+    """Per-call counts of RsPacing against restate.Resampler: 1-frame calls, tiny calls then a large one, a drain,
+    reset() mid-stream (the drain counters persist, so a second drain after a reset is dry), and a drain after a
+    reset before the first block."""
+    from oracle import restate
+    fi, fo = rates
+    r = restate.Resampler(fi, fo, 1, bw=bw)
+    p = RsPacing(fi, fo, bw)
+    L = r.in_len
+    script = ([("run", 1)] * 40 + [("run", 5)] * 200 + [("run", 3 * L + 17)] + [("reset", 0), ("run", L - 1), ("drain", 7)]
+              + [("drain", 1), ("drain", 4096)] * 3 + [("reset", 0), ("run", 1), ("run", 8192)] + [("drain", 1000)] * 3
+              + [("reset", 0), ("drain", 5)])
+    for op, f in script:
+        if op == "run":
+            assert p.run(f) == r.run(np.zeros((f, 1))).shape[0]
+        elif op == "reset":
+            p.reset()
+            r.reset()
+        else:
+            y = r.drain2(f)
+            assert p.drain(f) == (None if y is None else y.shape[0])
+    assert p.is_draining and p.drain_frames > 0

@@ -11,6 +11,13 @@ inputs, against an 80-bit long-double run of the same coefficients.  Bound per c
 err_gpu <= max(4 err_ref64, 64 u rms(truth)), where err_ref64 is the error of the reference's own FP64
 recurrence (restate.biquad_cascade) and u = 2^-53.
 
+Resample: the polyphase form against the long-double tap table and stream of accuracy.resample_truth, bound
+normalized RMS <= 1e-14 and max <= 1e-13 (scale = rms(x) ||G|| per channel), scaled up for very long tables
+(_table_factor).  Measured (H100 80GB HBM3, 400 W), worst per group: tap-table readback max 4.8e-15 ||G||; every
+DSP_B200_RS_TILE variant at tile edges 1.4e-15 / 7.5e-15; warps per CTA 1.4e-15 / 7.1e-15; the 15 ratios at
+bandwidth 0.7 2.8e-15 / 9.1e-15, at 0.99 1.0e-14 / 4.6e-14, at 0.999 1.5e-14 / 5.9e-14; stream shapes 6.0e-15 /
+2.6e-14 (6:1).  Tiles 1-3 agree bit for bit with each other, and so do tiles 4-7.
+
 Errors of each case are appended as JSON lines to the file DSP_B200_ACCURACY_LOG names, when it is set.
 """
 import json
@@ -20,7 +27,8 @@ import zlib
 import numpy as np
 import pytest
 
-from accuracy import H_MAX, biquad_within_ref, dyadic_signal, dyadic_taps, env, exact_conv, fir_nerr
+from accuracy import (H_MAX, RS_RATIOS, RsPacing, biquad_within_ref, dyadic_signal, dyadic_taps, env, exact_conv, fir_nerr,
+                      resample_taps_truth, resample_truth, rs_counts, rs_nerr, taps_norm)
 
 pytestmark = pytest.mark.gpu
 FIR_RMS, FIR_MAX = 1e-14, 1e-13
@@ -306,3 +314,347 @@ def test_biquad_per_channel_identity_sections_and_fused_neighbours(gpu_lib):
     ch.close()
     nxt.close()
     bq_check("per_channel_fused", got, x, coefs)
+
+
+# ------------------------------------------------------------------------------------------------------------
+# Resample
+# ------------------------------------------------------------------------------------------------------------
+RS_RMS, RS_MAX = 1e-14, 1e-13
+_G_CACHE = {}
+
+
+def _table_factor(gpu_lib, fi, fo, bw):
+    """max(1, sqrt(K / 8192)), K = sinc_len: what the stream bounds are multiplied by.  The device builds each tap as
+    a K-term cosine sum in FP64 (k_rs_table, after a K-bin DFT of the sinc).  Its error per tap stays below 5e-15
+    ||G|| (readback below), but an output sums in_len of those errors, and where they are correlated along the window
+    (a sine, a DC step) they add up: the FMA and tensor-core kernels, which sum in different orders, show identical
+    stream errors, so the table, not the accumulation, is what they measure.  Measured (H100 80GB HBM3, 400 W): at
+    most 2.8e-15 RMS up to K = 8000; 1.0e-14 RMS / 4.6e-14 max at K = 21504 (6:1, bandwidth 0.99); 1.5e-14 / 5.9e-14
+    at K = 71680 (2:1 and 1:2, bandwidth 0.999).  Up to K = 8192 (every ratio at the default bandwidth) the bounds
+    apply as they are."""
+    return max(1.0, np.sqrt(gpu_lib.resample_params(fi, fo, bw)["sinc_len"] / 8192.0))
+
+
+def _taps(fi, fo, bw):
+    if (fi, fo, bw) not in _G_CACHE:
+        _G_CACHE[(fi, fo, bw)] = resample_taps_truth(fi, fo, bw)
+    return _G_CACHE[(fi, fo, bw)]
+
+
+def _rs_chain(gpu_lib, fi, fo, C, bw, tile=None):
+    """A chain with one resampler; `tile` forces DSP_B200_RS_TILE for this operator (None: the default)."""
+    with env(DSP_B200_RS_TILE=tile):
+        return gpu_lib.Chain(fi, C).add_resample(fo, bw)
+
+
+def _plan(ch):
+    p = ch.describe()[0]
+    assert p["op"] == "resample", p
+    return p
+
+
+def _expect_tile(C, force):
+    """The variant resample.cu runs for `force` (0: none) on C channels."""
+    tile = 7 if C % 4 == 0 else 2 if C % 2 == 0 else 3
+    if 1 <= force <= 7 and not (((force == 1 or force >= 4) and C % 4) or (force == 2 and C % 2)):
+        tile = force
+    return tile, ("k_rs_poly" if tile <= 3 else "k_rs_mma" if tile == 4 else "k_rs_mma2")
+
+
+def _expect_warps(C, oframes, sms):
+    tiles = -(-oframes // 32)
+    return 4 if C >= 128 and tiles * -(-C // 128) >= 3 * sms else 2 if C >= 64 and tiles * -(-C // 64) >= 2 * sms else 1
+
+
+def rs_bases(fi, fo, bw, N, seed):
+    """[N, 5]: dyadic white noise; a 0.9 full-scale sine just inside the passband edge; a tone in the stopband (in the
+    transition band when upsampling, where the input has no stopband); a DC step 0 -> 0.9; +-0.5 at the input Nyquist."""
+    rng = np.random.default_rng(seed)
+    t = np.arange(N) / fi
+    mn = min(fi, fo)
+    x = np.zeros((N, 5))
+    x[:, 0] = dyadic_signal(rng, N, 1)[:, 0]
+    x[:, 1] = 0.9 * np.sin(2 * np.pi * 0.97 * bw * mn / 2 * t + 0.3)
+    f_stop = 0.5 * (mn / 2 + fi / 2) if fo < fi else 0.499 * fi
+    x[:, 2] = 0.9 * np.sin(2 * np.pi * f_stop * t + 1.1)
+    x[N // 3:, 3] = 0.9
+    x[:, 4] = 0.5 * (1 - 2 * (np.arange(N) % 2))
+    return x
+
+
+def _tiled(base, C):
+    return np.ascontiguousarray(base[:, np.arange(C) % base.shape[1]])
+
+
+def _check_stream(name, got, base, fi, fo, bw, rows=None, seed=0, factor=1.0):
+    """got [n_out, C] (channel c carries base c % 5): the first channels against the truth (on `rows` or, past 4000
+    outputs, on the first and last 200 and a seeded sample), the others bit for bit equal to them.  Returns the errors."""
+    C, k = got.shape[1], min(got.shape[1], base.shape[1])
+    for c in range(k, C):
+        assert np.array_equal(got[:, c], got[:, c % base.shape[1]]), (name, c)
+    G = _taps(fi, fo, bw)
+    if rows is None:
+        rows = np.arange(got.shape[0])
+        if rows.size > 4000:
+            rng = np.random.default_rng(seed)
+            rows = np.unique(np.concatenate([rows[:200], rows[-200:], rng.choice(rows, 3600, replace=False)]))
+    want = resample_truth(base[:, :k], fi, fo, bw, got.shape[0], rows=rows, G=G)
+    r, m = rs_nerr(got[rows, :k], want, base[:, :k], G)
+    _record("resample", name, rms=r, max=m)
+    assert r <= RS_RMS * factor and m <= RS_MAX * factor, (name, r, m, factor)
+    return r, m
+
+
+def _run_calls(ch, x, sizes):
+    outs, pos = [], 0
+    for f in sizes:
+        outs.append(ch.run(x[pos:pos + f]).copy())
+        pos += f
+    return outs
+
+
+def _drain(ch, block):
+    outs = []
+    while (y := ch.drain(block)) is not None:
+        outs.append(y)
+    return outs
+
+
+RS_READBACK = [(r, bw) for bw in (0.7, 0.99) for r in [(44100, 48000), (48000, 44100), (44100, 192000), (8000, 48000),
+                                                        (48000, 8000), (48000, 96000)]] + [((96000, 48000), 0.999), ((48000, 96000), 0.999)]
+
+
+@pytest.mark.parametrize("rates,bw", RS_READBACK, ids=lambda v: "%d-%d" % v if isinstance(v, tuple) else "bw%s" % v)
+def test_resample_tap_table_readback(gpu_lib, rates, bw):
+    """Channel c carries one unit impulse, at input row r0 + c (c < d, r0 >= 2 in_len): every emitted output is then
+    exactly one tap, G[(m d) mod n][floor(m d / n) - r0 - c], and every other product is an exact zero, so the d
+    channels read the device's whole table back.  Each tap against the long-double table, and exactly 0.0 wherever
+    the window misses the impulse; on C = d channels through the FMA kernel (DSP_B200_RS_TILE=3) and on d rounded up
+    to a multiple of 4 through the tensor-core default, which must read the same bits.  Bound max |dG| <= 1e-14 ||G||
+    times _table_factor."""
+    fi, fo = rates
+    G = _taps(fi, fo, bw)
+    n, in_len = G.shape
+    nG = taps_norm(G)
+    p = gpu_lib.resample_params(fi, fo, bw)
+    d, out_delay = p["d"], p["out_delay"]
+    r0 = 2 * in_len
+    N = r0 + 2 * d + in_len + 64
+    got = []
+    for C, tile, kernel in ((d, 3, "k_rs_poly"), (d + (-d) % 4, None, "k_rs_mma2")):
+        x = np.zeros((N, C))
+        x[r0 + np.arange(C), np.arange(C)] = 1.0
+        ch = _rs_chain(gpu_lib, fi, fo, C, bw, tile)
+        y = np.concatenate(_run_calls(ch, x, [4096] * (N // 4096) + [N % 4096]) + _drain(ch, 4096))
+        assert _plan(ch)["kernel"] == kernel
+        ch.close()
+        m = out_delay + np.arange(y.shape[0])
+        ph, ih = (m * d) % n, (m * d) // n
+        t = ih[:, None] - r0 - np.arange(C)[None, :]
+        inside = (t >= 0) & (t < in_len)
+        cover = np.zeros((n, in_len), dtype=bool)
+        cover[np.broadcast_to(ph[:, None], t.shape)[inside], t[inside]] = True
+        assert cover.all(), "the impulses do not reach every tap"
+        assert np.all(y[~inside] == 0.0), (C, "nonzero output where the window misses the impulse")
+        want = G.astype(np.float64)[np.broadcast_to(ph[:, None], t.shape)[inside], t[inside]]
+        err = float(np.max(np.abs(y[inside] - want))) / nG
+        _record("resample", "readback/%d-%d/bw%s/C%d" % (fi, fo, bw, C), max=err)
+        assert err <= 1e-14 * _table_factor(gpu_lib, fi, fo, bw), (C, err)
+        got.append(y[:, :d])
+    assert np.array_equal(got[0], got[1]), "the FMA and tensor-core kernels read different taps"
+
+
+RS_SHAPES = {"mma": [4, 36, 64, 68, 124, 132, 260], "pair": [2, 66, 130], "single": [1, 33, 129]}
+
+
+@pytest.mark.parametrize("shape", list(RS_SHAPES))
+def test_resample_every_variant_at_channel_tile_edges(gpu_lib, shape):
+    """44100 -> 48000 with DSP_B200_RS_TILE = 0 (default) and 1..7 on channel counts at the tile edges of each kernel
+    (tensor-core shapes: a partly filled warp, CTA column or last 128 channels; pair and single-channel shapes for the
+    FMA kernel, on which a forced tile the count cannot use falls back to the default), calls of 1, 7, in_len - 1,
+    in_len, in_len + 1 and 4096 frames, then the drain.  describe() names the kernel and tile that ran; counts as
+    rs_counts replays them; the five base signals against the truth, their copies in the other channels bit for bit;
+    and within each family (tiles 1-3 on the FMA kernel, 4-7 on the tensor cores) every tile gives the same bits: an
+    output meets the same products in the same order, and the leading zero taps add exact zeros."""
+    fi, fo, bw = 44100, 48000, 0.939
+    in_len = gpu_lib.resample_params(fi, fo)["in_len"]
+    sizes = [1, 7, in_len - 1, in_len, in_len + 1, 4096, 1, 4096]
+    N = sum(sizes)
+    base = rs_bases(fi, fo, bw, N, seed=7)
+    counts, drains = rs_counts(fi, fo, sizes, 1000, bw)
+    worst = (0.0, 0.0)
+    for C in RS_SHAPES[shape]:
+        x = _tiled(base, C)
+        family = {}
+        for force in range(8):
+            tile, kernel = _expect_tile(C, force)
+            ch = _rs_chain(gpu_lib, fi, fo, C, bw, force)
+            outs = _run_calls(ch, x, sizes)
+            plan = _plan(ch)
+            dr = _drain(ch, 1000)
+            ch.close()
+            assert (plan["force_tile"], plan["tile"], plan["kernel"]) == (force, tile, kernel), (C, force, plan)
+            assert [o.shape[0] for o in outs] == counts and [o.shape[0] for o in dr] == drains, (C, force)
+            got = np.concatenate(outs + dr)
+            fam = tile >= 4
+            if fam in family:
+                assert np.array_equal(got, family[fam]), (C, force, "differs from another tile of its family")
+                continue
+            family[fam] = got
+            e = _check_stream("variants/C%d/tile%d" % (C, tile), got, base, fi, fo, bw)
+            worst = (max(worst[0], e[0]), max(worst[1], e[1]))
+    _record("resample", "variants/%s/worst" % shape, rms=worst[0], max=worst[1])
+
+
+@pytest.mark.parametrize("C", [68, 132, 260])
+def test_resample_warps_per_cta(gpu_lib, C):
+    """The tensor-core kernels' warps per CTA (4, 2 or 1, from the channel count, the output tiles of the call and
+    the device's SM count) on 68, 132 and 260 channels (the last 64- or 128-channel column partly filled), for tiles
+    4-7, with call sizes scaled by the SM count so that each call reaches a known choice: describe() reports the
+    choice resample.cu's formula makes for the frames the call emitted, and every choice the channel count allows is
+    reached.  Values against the truth, copies bit for bit."""
+    import torch
+    sms = torch.cuda.get_device_properties(0).multi_processor_count
+    fi, fo, bw = 44100, 48000, 0.939
+    sizes = [k * sms for k in (4, 16, 26, 36, 50, 64)] + [3]
+    N = sum(sizes)
+    base = rs_bases(fi, fo, bw, N, seed=C)
+    x = _tiled(base, C)
+    allowed = {1, 2, 4} if C >= 128 else {1, 2}
+    ref = None
+    for force in (4, 5, 6, 7):
+        ch = _rs_chain(gpu_lib, fi, fo, C, bw, force)
+        outs, reached = [], set()
+        pos = 0
+        for f in sizes:
+            outs.append(ch.run(x[pos:pos + f]).copy())
+            pos += f
+            if outs[-1].shape[0]:
+                plan = _plan(ch)
+                w = _expect_warps(C, outs[-1].shape[0], sms)
+                assert (plan["tile"], plan["warps"]) == (force, w), (force, outs[-1].shape[0], plan)
+                assert plan["depth"] == (1 if force == 4 else 3 if force == 6 and w == 4 else 2), plan
+                reached.add(w)
+        ch.close()
+        assert reached == allowed, (force, reached)
+        got = np.concatenate(outs)
+        if ref is None:
+            ref = got
+            _check_stream("warps/C%d" % C, got, base, fi, fo, bw)
+        else:
+            assert np.array_equal(got, ref), force
+
+
+def _rates_id(r):
+    return "%d-%d" % r
+
+
+@pytest.mark.parametrize("bw", [0.7, 0.99])
+@pytest.mark.parametrize("rates", RS_RATIOS, ids=_rates_id)
+def test_resample_ratios_and_bandwidths(gpu_lib, rates, bw):
+    """The 15 ratios of test_resample_ratios at bandwidths 0.7 and 0.99 (`resample 0.99 48000`), on 5 channels (the
+    FMA kernel) and 8 (tensor cores), ragged calls and the drain; counts as rs_counts replays them, the five inputs
+    against the truth."""
+    _ratio_case(gpu_lib, rates, bw)
+
+
+@pytest.mark.parametrize("rates", [(96000, 48000), (48000, 96000)], ids=_rates_id)
+def test_resample_bandwidth_0_999(gpu_lib, rates):
+    """Bandwidth 0.999 at 2:1 and 1:2: in_len is tens of thousands (long k_end loops, many tap chunks, a large padded
+    table) while the table itself is cheap (n <= 2); checked on a seeded sample of outputs."""
+    _ratio_case(gpu_lib, rates, 0.999, sample=2000)
+
+
+def _ratio_case(gpu_lib, rates, bw, sample=None):
+    fi, fo = rates
+    in_len = gpu_lib.resample_params(fi, fo, bw)["in_len"]
+    rng = np.random.default_rng(fi + fo)
+    sizes = [1, 7, in_len - 1, in_len, in_len + 1]
+    while sum(sizes) < 3 * in_len + 2000:
+        sizes.append(int(rng.integers(1, 4097)))
+    N = sum(sizes)
+    base = rs_bases(fi, fo, bw, N, seed=fi + fo)
+    counts, drains = rs_counts(fi, fo, sizes, 4096, bw)
+    rows, ref = None, None
+    for C, kernel in ((5, "k_rs_poly"), (8, "k_rs_mma2")):
+        ch = _rs_chain(gpu_lib, fi, fo, C, bw)
+        outs = _run_calls(ch, _tiled(base, C), sizes)
+        assert _plan(ch)["kernel"] == kernel
+        dr = _drain(ch, 4096)
+        ch.close()
+        assert [o.shape[0] for o in outs] == counts and [o.shape[0] for o in dr] == drains, C
+        got = np.concatenate(outs + dr)
+        if sample and rows is None:
+            rows = np.unique(np.concatenate([np.arange(100), got.shape[0] - 1 - np.arange(100),
+                                             rng.choice(got.shape[0], sample, replace=False)]))
+        _check_stream("ratios/%d-%d/bw%s/C%d" % (fi, fo, bw, C), got, base, fi, fo, bw, rows=rows, seed=fi,
+                      factor=_table_factor(gpu_lib, fi, fo, bw))
+
+
+def _pacing_to(fi, fo, bw, target, block=1000):
+    """Smallest stream of `block`-frame calls (from 5 in_len on) after which in_buf_pos == target."""
+    p0 = RsPacing(fi, fo, bw)
+    N = 5 * p0.in_len
+    while True:
+        p = RsPacing(fi, fo, bw)
+        sizes = [block] * (N // block) + ([N % block] if N % block else [])
+        for f in sizes:
+            p.run(f)
+        if p.in_buf_pos == target:
+            return sizes
+        N += 1
+
+
+@pytest.mark.parametrize("rates", [(44100, 48000), (48000, 8000)], ids=_rates_id)
+@pytest.mark.parametrize("case", ["first_block", "wrap_then_grow", "reset", "drain_end", "drain_reset_drain"])
+def test_resample_stream_shapes(gpu_lib, rates, case):
+    """Per-call counts against rs_counts / RsPacing and values against the truth, on 5 (FMA) and 8 (tensor-core)
+    channels: calls summing to in_len - 1, in_len and in_len + 1 before the first output; 2000 calls of 5 frames (the
+    ring wraps many times), one of 50000 (the ring grows after a wrap) and small calls again; reset() mid-stream, then
+    1 frame and 8192; the drain after streams that end with in_buf_pos = 0, in_len - 1 and mid-block, polled 1 (when
+    upsampling), 7 and 4096 frames at a time; drain, reset(), the stream again, and a second drain, which is dry because the drain
+    counters persist across reset() as in the reference."""
+    fi, fo = rates
+    bw = 0.939
+    L = gpu_lib.resample_params(fi, fo)["in_len"]
+    runs = []   # (name, sizes, drain poll or None); a None entry in `runs` is a reset()
+    if case == "first_block":
+        for k, pre in enumerate(([L - 1], [L - 3, 2], [L], [L - 1, 1], [L + 1], [1, L - 1, 1])):
+            runs.append([("pre%d" % k, pre + [7, L, 4096, 1], 4096)])
+    elif case == "wrap_then_grow":
+        runs.append([("wrap_grow", [5] * 2000 + [50000] + [3] * 300, None)])
+    elif case == "reset":
+        runs.append([("before", [1000] * 3 + [L // 2], None), None, ("after", [1, 8192], 7)])
+    elif case == "drain_end":
+        for target in (0, L - 1, L // 2):
+            for poll in (1, 7, 4096) if fo > fi else (7, 4096):   # 1-frame polls at 6:1: mostly empty host calls
+                runs.append([("end%d/poll%d" % (target, poll), _pacing_to(fi, fo, bw, target), poll)])
+    else:
+        runs.append([("first", [3000, 1, 2000], 1000), None, ("again", [2500, 4096], 1000)])
+    for C in (5, 8):
+        for seq in runs:
+            ch = _rs_chain(gpu_lib, fi, fo, C, bw)
+            pacing = RsPacing(fi, fo, bw)
+            for step in seq:
+                if step is None:
+                    ch.reset()
+                    pacing.reset()
+                    continue
+                name, sizes, poll = step
+                N = sum(sizes)
+                base = rs_bases(fi, fo, bw, N, seed=N + C)
+                outs = _run_calls(ch, _tiled(base, C), sizes)
+                assert [o.shape[0] for o in outs] == [pacing.run(f) for f in sizes], name
+                if poll:
+                    dr = _drain(ch, poll)
+                    want = []
+                    while (o := pacing.drain(poll)) is not None:
+                        want.append(o)
+                    assert [o.shape[0] for o in dr] == want, name
+                    outs += dr
+                got = np.concatenate(outs)
+                if case == "drain_reset_drain" and name == "again":
+                    assert want == [], "the second drain after reset() must be dry"
+                if got.shape[0]:
+                    _check_stream("stream/%d-%d/%s/%s/C%d" % (fi, fo, case, name, C), got, base, fi, fo, bw)
+            ch.close()
