@@ -1436,18 +1436,24 @@ struct FirOp : Op {
 	double *d_lo = nullptr, *d_hi = nullptr;
 	long abs_pos = 0;                    // frames consumed so far (level-0 block = abs_pos / B0, offset = abs_pos % B0)
 	bool pre_valid = false;
+	// which paths the stream took since the last plan() (describe() "paths"): level-0 blocks completed by the fused kernel
+	// (per-channel form / cluster form), the pipeline kernel, the bulk form and the general path (forward, MAC, inverse),
+	// and launches of the head kernel (ragged calls)
+	long n_fused = 0, n_cluster = 0, n_pipe = 0, n_bulk = 0, n_general = 0, n_head = 0;
 
 	const char *name() const override { return "fir"; }
 
 	std::string describe() const override
 	{
-		char buf[512];
+		char buf[1024];
 		int n = snprintf(buf, sizeof(buf), "{\"op\":\"fir\",\"taps\":%ld,\"n_sel\":%d,\"filter_channels\":%d,\"latency\":%ld,\"planned\":%d,\"levels\":[",
 		                 filter_frames, n_sel, fc, latency, planned ? 1 : 0);
 		for (int l = 0; l < n_levels && n < (int) sizeof(buf) - 64; ++l)
 			n += snprintf(buf + n, sizeof(buf) - n, "%s{\"B\":%d,\"P\":%d}", l ? "," : "", lv[l].B, lv[l].P);
-		snprintf(buf + n, sizeof(buf) - n, "],\"t_batch\":%d,\"t_far\":%d,\"far_e\":%d,\"far_classes\":%d,\"stagger\":%d,\"merge\":%d,\"tail_pf\":%d,\"bulk\":%d,\"pipe\":%d,\"pipe_pf\":%d}",
-		         t_batch, t_far, far_e, far_classes, stagger ? 1 : 0, merge_tail ? 1 : 0, tail_pf, nb_max, use_pipe ? 1 : 0, pipe_pf);
+		n += snprintf(buf + n, sizeof(buf) - n, "],\"t_batch\":%d,\"t_far\":%d,\"far_e\":%d,\"far_classes\":%d,\"stagger\":%d,\"merge\":%d,\"tail_pf\":%d,\"bulk\":%d,\"pipe\":%d,\"pipe_pf\":%d,",
+		              t_batch, t_far, far_e, far_classes, stagger ? 1 : 0, merge_tail ? 1 : 0, tail_pf, nb_max, use_pipe ? 1 : 0, pipe_pf);
+		snprintf(buf + n, sizeof(buf) - n, "\"replans\":%d,\"paths\":{\"fused\":%ld,\"cluster\":%ld,\"pipe\":%ld,\"bulk\":%ld,\"general\":%ld,\"head\":%ld}}",
+		         replans, n_fused, n_cluster, n_pipe, n_bulk, n_general, n_head);
 		return buf;
 	}
 
@@ -1505,6 +1511,7 @@ struct FirOp : Op {
 		int b = 64;
 		while (b * 2 <= hint && b < FIR_MAX_B) b *= 2;
 		B0 = b;
+		n_fused = n_cluster = n_pipe = n_bulk = n_general = n_head = 0;
 		const long T = filter_frames;
 		// level plan (see the header comment)
 		n_levels = 0;
@@ -2028,6 +2035,7 @@ struct FirOp : Op {
 		}
 		CUDA_TRY(cudaMemcpyAsync(L.carry, d_hi + (size_t) (nb - 1) * n_sel * B0, (size_t) n_sel * B0 * sizeof(double), cudaMemcpyDeviceToDevice, st), return -1);
 		L.blk += nb;
+		n_bulk += nb;
 		pre_valid = false;
 		return 0;
 	}
@@ -2172,11 +2180,13 @@ struct FirOp : Op {
 					f.stats = d_stats;
 					if (launch_pipe(B0, f, st)) return -1;
 					++L0.blk;
+					++n_pipe;
 					last_block_piped = true;
 				}
 				else if (use_pipe) {
 					// a whole block that cannot use the direct form (never happens today: direct_io is a plan-time switch)
 					if (level_block(L0, d_ytmp, B0, INV_OUT | INV_UPDATE_CARRY, st)) return -1;
+					++n_general;
 				}
 				else if (L0.P <= 2 || tail_pf == 2) {
 					L0Args f = {};
@@ -2212,8 +2222,13 @@ struct FirOp : Op {
 						CUDA_TRY(cudaStreamWaitEvent(st, ev_hot_out, 0), return -1);
 					}
 					++L0.blk;
+					if (f.cluster_io) ++n_cluster;
+					else ++n_fused;
 				}
-				else if (level_block(L0, d_ytmp, B0, INV_OUT | INV_UPDATE_CARRY, st)) return -1;
+				else {
+					if (level_block(L0, d_ytmp, B0, INV_OUT | INV_UPDATE_CARRY, st)) return -1;
+					++n_general;
+				}
 				if (!direct) {
 					side_wait(abs_pos, st);
 					LAUNCH(k_fir_unstash, tgrid_full, 256, 0, st, d_ytmp, (long) B0, pend, d, dstride, dmap, B0, n_sel);
@@ -2226,11 +2241,13 @@ struct FirOp : Op {
 				side_wait(abs_pos, st);
 				LAUNCH(k_fir_head, grid, 128, 0, st, d_hist, hist_len, blk_off, d_pre, d_h0, (fc == 1) ? 0L : (long) B0, pend,
 				       d, dstride, dmap, B0, pos, seg);
+				++n_head;
 				if (pos + seg == B0) {
 					// block complete: X into the FDL, carry = IRFFT(S)[B:2B) (its first half has been emitted already)
 					last_block_piped = false;
 					if (wait_batch_for(L0.blk, st)) return -1;
 					if (level_block(L0, nullptr, 0, INV_UPDATE_CARRY, st)) return -1;
+					++n_general;
 					pre_valid = false;
 				}
 			}

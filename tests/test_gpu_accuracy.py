@@ -6,6 +6,15 @@ multiple of 64 taps -- every partition boundary of every plan), through every pl
 Bound: normalized RMS <= 1e-14, normalized max <= 1e-13 (scale = rms(x) ||h||_2 per channel).  Measured on an
 H100 80GB HBM3 (400 W limit), worst over every FIR case below: RMS 4.8e-16, max 3.3e-15.
 
+FIR plan edges (test_fir_plan_edges_exact and the two tests after it): every boundary FirOp::plan() draws, each case
+asserting its plan and which paths ran, in whole blocks and then ragged calls after reset().  Measured on an H100
+80GB HBM3 (700 W limit), worst normalized RMS / max per group: fused kernel without tail (P = 1, 2) 4.7e-16 /
+2.7e-15; tail, batch and stagger thresholds 4.6e-16 / 2.7e-15; far tier at P = 47 / 48 4.7e-16 / 2.7e-15; batch
+depths 6 and 8 4.2e-16 / 2.7e-15; pipeline kernel with and without batch 4.6e-16 / 2.5e-15; multi-level 4.3e-16 /
+3.0e-15; eight levels 4.4e-16 / 2.8e-15; bulk 4.9e-16 / 2.9e-15; FFT tiles at CPB +- 1 4.5e-16 / 2.3e-15; cluster
+fall-backs (selectors, misaligned device buffers) 4.7e-16 / 2.9e-15; latency ring 4.5e-16 / 2.6e-15; re-planning
+4.2e-16 / 2.4e-15.
+
 Biquad: ill-conditioned sections (poles near z = 1: corners down to 5 Hz at up to 192 kHz) on large, slow
 inputs, against an 80-bit long-double run of the same coefficients.  Bound per channel:
 err_gpu <= max(4 err_ref64, 64 u rms(truth)), where err_ref64 is the error of the reference's own FP64
@@ -187,6 +196,281 @@ def test_fir_block_io_and_stream_shapes_exact(gpu_lib, case, family):
     r, m = max(w[0] for w in worst), max(w[1] for w in worst)
     _record("fir", "%s/%s" % (case, family), rms=r, max=m)
     assert r <= FIR_RMS and m <= FIR_MAX, (case, family, r, m, plan)
+
+
+# Plan edges: every boundary FirOp::plan() draws, each case with the plan it must make.  A planner change that moves
+# a case off its edge fails the plan assertion instead of quietly testing something else.
+FIR_EDGES = {}
+PATHS = ("fused", "cluster", "pipe", "bulk", "general")   # describe()["paths"]: level-0 blocks per path ("head": launches)
+
+
+def _fir_plan(levels, **kw):
+    """The describe() fields a case must show: levels [(B, P), ...]; tail_pf, t_batch, t_far, stagger, pipe and
+    pipe_pf are 0 and bulk (blocks per bulk launch) is 1 unless given."""
+    p = dict(levels=[{"B": B, "P": P} for B, P in levels], tail_pf=0, t_batch=0, t_far=0, stagger=0, bulk=1, pipe=0, pipe_pf=0)
+    p.update(kw)
+    return p
+
+
+def _edge(group, name, taps, C, hint, plan, envs=None, sel=None, latency=0, rising=False, short=False, lead=(), call=None):
+    """One case: `hint` is the block hint (level 0's B), `call` the frames per call of the whole-block pass (default
+    B0), `lead` the first calls of the ragged pass, `rising` adds the rising family (threshold cases), `short` runs a
+    stream shorter than the filter."""
+    FIR_EDGES["%s/%s" % (group, name)] = dict(taps=taps, C=C, hint=hint, plan=plan, envs=envs or {}, sel=sel, latency=latency,
+                                              rising=rising, short=short, lead=tuple(lead), call=call)
+
+
+def _ladder(B0, last_P, top=4096):
+    """Multi-level plans: level 0 (B0, P = 2), one partition on every level up to `top`, `last_P` on the last."""
+    lv, B = [(B0, 2)], 2 * B0
+    while B < top:
+        lv.append((B, 1))
+        B *= 2
+    return lv + [(top, last_P)]
+
+
+# single level, fused kernel, no tail: P = 1 up to T = B, P = 2 from one tap more
+for _B in (64, F2, F4):
+    for _T, _P in ((1, 1), (2, 1), (_B - 1, 1), (_B, 1), (_B + 1, 2), (2 * _B, 2)):
+        _edge("fused", "B%d_T%d" % (_B, _T), _T, 3 if _B == 64 else 4 if _B == F2 else 5, _B, _fir_plan([(_B, _P)]))
+# single level, tail thresholds: the tail from P = 3, the batch from P = 11, the stagger from P = 22
+for _B in (F2, F4):
+    for _k, _P, _kw, _thr in ((2, 3, {}, False), (10, 10, {}, False), (10, 11, dict(t_batch=4), True),
+                              (21, 21, dict(t_batch=4), False), (21, 22, dict(t_batch=4, stagger=1), True)):
+        _T = _k * _B + (_P - _k)
+        _edge("tail", "B%d_P%d" % (_B, _P), _T, 4 if _B == F2 else 5, _B, _fir_plan([(_B, _P)], tail_pf=2, **_kw), rising=_thr)
+_edge("tail", "B2048_P22_short", 21 * F2 + 1, 4, F2, _fir_plan([(F2, 22)], tail_pf=2, t_batch=4, stagger=1), short=True)
+# far tier from P = 48 (whole launches: no stagger)
+_edge("far", "P47", 47 * F2, 4, F2, _fir_plan([(F2, 47)], tail_pf=2, t_batch=4, stagger=1))
+_edge("far", "P48", 47 * F2 + 1, 4, F2, _fir_plan([(F2, 48)], tail_pf=2, t_batch=4, t_far=8), rising=True)
+# batch depths 6 and 8: the batch from P = 2 T + 3
+for _tb, _k in ((6, 14), (8, 18)):
+    _edge("depth", "T%d_P%d" % (_tb, _k), _k * F2, 4, F2, _fir_plan([(F2, _k)], tail_pf=2), envs=dict(DSP_B200_FIR_T=_tb))
+    _edge("depth", "T%d_P%d" % (_tb, _k + 1), _k * F2 + 1, 4, F2, _fir_plan([(F2, _k + 1)], tail_pf=2, t_batch=_tb),
+          envs=dict(DSP_B200_FIR_T=_tb), rising=True)
+# pipeline kernel: it sums every partition itself (pipe_pf = P) until the batch starts at P = 11
+for _B in (F2, F4):
+    for _T, _P, _kw in ((2 * _B + 1, 3, dict(pipe_pf=3)), (3 * _B + 1, 4, dict(pipe_pf=4)), (10 * _B, 10, dict(pipe_pf=10)),
+                        (10 * _B + 1, 11, dict(pipe_pf=6, t_batch=4))):
+        _edge("pipe", "B%d_P%d" % (_B, _P), _T, 4, _B, _fir_plan([(_B, _P)], tail_pf=2, pipe=1, **_kw),
+              envs=dict(DSP_B200_FIR_PIPE=1), rising=_P == 11)
+# multi-level: an upper level holding one tap, the last level (4096) at P = 1 and 2 (the tail starts), 9 and 10 (the batch)
+for _B0 in (64, 128, 256, 512, 1024):
+    _C = {64: 3, 128: 4, 256: 5, 512: 4, 1024: 2}[_B0]
+    _edge("multi", "B%d_T%d" % (_B0, 2 * _B0 + 1), 2 * _B0 + 1, _C, _B0, _fir_plan([(_B0, 2), (2 * _B0, 1)]))
+    _edge("multi", "B%d_T%d" % (_B0, 4 * _B0), 4 * _B0, _C, _B0, _fir_plan([(_B0, 2), (2 * _B0, 1)]))
+    _edge("multi", "B%d_T%d" % (_B0, 4 * _B0 + 1), 4 * _B0 + 1, _C, _B0, _fir_plan([(_B0, 2), (2 * _B0, 1), (4 * _B0, 1)]))
+    _edge("multi", "B%d_T8192" % _B0, 8192, _C, _B0, _fir_plan(_ladder(_B0, 1)))
+    _edge("multi", "B%d_T8193" % _B0, 8193, _C, _B0, _fir_plan(_ladder(_B0, 2), tail_pf=1), rising=True)
+    _edge("multi", "B%d_T40960" % _B0, 40960, _C, _B0, _fir_plan(_ladder(_B0, 9), tail_pf=1))
+    _edge("multi", "B%d_T40961" % _B0, 40961, _C, _B0, _fir_plan(_ladder(_B0, 10), tail_pf=1, t_batch=4), rising=True)
+_edge("multi", "B256_T40961_short", 40961, 5, 256, _fir_plan(_ladder(256, 10), tail_pf=1, t_batch=4), short=True)
+# the most levels a plan has (FIR_MAX_LEVELS = 8): seven upper levels feed `pend`
+_edge("levels", "B64_cap8192", 131072, 2, 64, _fir_plan(_ladder(64, 15, top=8192), tail_pf=1, t_batch=4),
+      envs=dict(DSP_B200_FIR_LEVEL_CAP=8192), rising=True)
+# bulk form: off at P = 2, from P = 3; calls that bring 2, 3 + 5 frames, 4 and 9 blocks, then 1 and B - 1 frames
+_BULK_LEAD = (1, 8191, 2 * 8192, 3 * 8192 + 5, 4 * 8192, 9 * 8192, 1, 8191)
+for _hint, _nb in ((16384, 2), (32768, 4)):
+    _edge("bulk", "hint%d_P2" % _hint, 16384, 3, _hint, _fir_plan([(8192, 2)]), lead=_BULK_LEAD, call=_hint)
+    _edge("bulk", "hint%d_P3" % _hint, 16385, 3, _hint, _fir_plan([(8192, 3)], bulk=_nb), lead=_BULK_LEAD, call=_hint, rising=True)
+    _edge("bulk", "hint%d_P10" % _hint, 10 * 8192, 3, _hint, _fir_plan([(8192, 10)], bulk=_nb), lead=_BULK_LEAD, call=_hint)
+# FFT tiles: CPB = 256 / (B / 16) channels per CTA; one channel less and one more
+for _B0, _cpb in ((64, 64), (128, 32), (256, 16), (512, 8), (1024, 4)):
+    for _C in (_cpb - 1, _cpb + 1):
+        _edge("cpb", "B%d_C%d" % (_B0, _C), 2 * _B0 + 1, _C, _B0, _fir_plan([(_B0, 2), (2 * _B0, 1)]))
+_edge("cpb", "B2048_C3", F2 + 1, 3, F2, _fir_plan([(F2, 2)]))
+# the fused kernel's cluster form takes 4 contiguous selected channels from an even one: an odd start and a
+# count that is no multiple of 4 fall back to the per-channel form
+for _B in (F2, F4):
+    for _P in (2, 3):
+        _pl = _fir_plan([(_B, _P)], tail_pf=2 if _P == 3 else 0)
+        _T = (_P - 1) * _B + 1
+        _edge("cluster", "B%d_P%d_sel1-4of6" % (_B, _P), _T, 6, _B, _pl, sel=[1 <= c <= 4 for c in range(6)])
+        _edge("cluster", "B%d_P%d_sel2-9of10" % (_B, _P), _T, 10, _B, _pl, sel=[2 <= c <= 9 for c in range(10)])
+        _edge("cluster", "B%d_P%d_all5" % (_B, _P), _T, 5, _B, _pl)
+# fir's latency ring: latencies around the call size, calls shorter and longer than the latency, 1-frame calls
+for _B0 in (64, F4):
+    for _T in (17, 255):
+        _pl = _fir_plan([(64, 1)] if _B0 == 64 and _T == 17 else [(64, 2), (128, 1)] if _B0 == 64 else [(F4, 1)])
+        for _lat in sorted({1, 17, _B0 - 1, _B0, _B0 + 1, 3 * _B0 + 5}):
+            _edge("latency", "B%d_T%d_lat%d" % (_B0, _T, _lat), _T, 3, _B0, _pl, latency=_lat,
+                  lead=(1, 1, max(_lat - 1, 1), _lat, _lat + 1, 1, 2 * _lat + 3, 1, 1, 3 * _lat, 5),
+                  envs=dict(DSP_B200_FIR_NO_REPLAN=1))   # calls longer than 2 B0 keep this plan
+
+
+def _ragged_sizes(rng, N, B, lead=()):
+    """Call sizes summing to N: `lead`, then from an aligned start B - 1, B, B + 1; B - 3 and six 1-frame calls across
+    a block boundary; B - 6 and B + 6 (from offset B - 3 across two boundaries); then seeded sizes.  While the
+    stream is young enough to be replayed (16384 frames) every call stays below 2 B, which would re-plan."""
+    sizes = list(lead)
+    pos = sum(sizes)
+    if pos % B:
+        sizes.append(B - pos % B)
+    sizes += [B - 1, B, B + 1, B - 3] + [1] * 6 + [B - 6, B + 6]
+    pos = sum(sizes)
+    while pos < N:
+        top = 2 * B - 1 if pos < 16384 + 2 * B else 4 * B + 7
+        f = min(int(rng.integers(1, top + 1)), N - pos)
+        sizes.append(f)
+        pos += f
+    return sizes
+
+
+def _run_sizes(ch, x, sizes):
+    return np.concatenate([o.copy() for o in _run_calls(ch, x, sizes)])
+
+
+def _check_plan(p, want, case):
+    for k, v in want.items():
+        assert p[k] == v, (case, k, p[k], v, p)
+
+
+def _edge_mixes(case):
+    return ["flat-shared", "comb-channel"] + (["rising-shared"] if FIR_EDGES[case]["rising"] else [])
+
+
+@pytest.mark.parametrize("case,mix", [(c, m) for c in FIR_EDGES for m in _edge_mixes(c)])
+def test_fir_plan_edges_exact(gpu_lib, case, mix):
+    """Every boundary of FirOp::plan() against the exact convolution, with the plan each case must make asserted
+    (describe()), in two passes of one chain: whole aligned blocks, then reset() and ragged calls (_ragged_sizes).
+    describe()["paths"] must show which path each pass took.  Streams of at least 2 R + 3 blocks of the last level
+    (R: FDL rows), so that every FDL and V-slot ring wraps; the `short` cases stop before the filter's length.  Taps
+    flat and shared by all channels, comb and per channel, and rising and shared on threshold cases.  Measured
+    (H100 80GB HBM3, 700 W): see the module docstring."""
+    e = FIR_EDGES[case]
+    family, taps_mode = mix.split("-")
+    T, C, hint, sel, lat, want_plan = e["taps"], e["C"], e["hint"], e["sel"], e["latency"], e["plan"]
+    n_sel = C if sel is None else sum(sel)
+    B0 = want_plan["levels"][0]["B"]
+    Bl, Pl = want_plan["levels"][-1]["B"], want_plan["levels"][-1]["P"]
+    R = Pl + want_plan["bulk"] - 1
+    N = max((2 * R + 3) * Bl, 16 * B0, 8 * lat + 4 * B0, sum(e["lead"]) + 8 * B0) + 77
+    if e["short"]:
+        N = T - 3 * B0 - 5
+    rng = np.random.default_rng(zlib.crc32((case + mix).encode()))
+    h = ir_family(family, T, 1 if taps_mode == "shared" else n_sel, seed=T)
+    x = dyadic_signal(rng, N, C)
+    want = exact_conv(x, h, H_SHIFT, selector=sel, latency=lat)
+    with env(**e["envs"]):
+        ch = gpu_lib.Chain(48000, C).add_fir(h if h.shape[1] > 1 else h[:, 0], selector=sel, latency=lat, block_hint=hint)
+        call = e["call"] or B0
+        NA = N // call * call
+        got_a = _run_sizes(ch, x[:NA], [call] * (NA // call))
+        pa = ch.describe()[0]
+        ch.reset()
+        got_b = _run_sizes(ch, x, _ragged_sizes(rng, N, B0, e["lead"]))
+        pb = ch.describe()[0]
+    ch.close()
+    _check_plan(pa, want_plan, case)
+    _check_plan(pb, want_plan, case)
+    # whole aligned blocks: one path for all of them
+    # (the cluster form: B0 >= 2048, an even channel count, selected channels contiguous -- as every selector here is --
+    # in fours from an even one)
+    cluster = B0 >= 2048 and C % 2 == 0 and n_sel % 4 == 0 and (sel is None or sel.index(True) % 2 == 0)
+    path =("pipe" if want_plan["pipe"] else "bulk" if want_plan["bulk"] > 1 else
+            ("cluster" if cluster else "fused") if want_plan["levels"][0]["P"] <= 2 or want_plan["tail_pf"] == 2 else "general")
+    assert pa["paths"] == dict({k: 0 for k in PATHS + ("head",)}, **{path: NA // B0}), (case, path, pa["paths"])
+    # ragged calls: the head kernel and the general path, every block by exactly one path
+    d = {k: pb["paths"][k] - pa["paths"][k] for k in PATHS + ("head",)}
+    assert d["head"] > 0 and d["general"] > 0 and sum(d[k] for k in PATHS) == N // B0, (case, d)
+    if want_plan["bulk"] > 1:
+        assert d["bulk"] > 0, (case, d)
+    if sel is not None:
+        for c in range(C):
+            if not sel[c]:
+                assert np.array_equal(got_a[:, c], x[:NA, c]) and np.array_equal(got_b[:, c], x[:, c]), (case, c)
+    ra, ma = fir_nerr(got_a, want[:NA], x[:NA], h, selector=sel)
+    rb, mb = fir_nerr(got_b, want, x, h, selector=sel)
+    r, m = max(ra, rb), max(ma, mb)
+    _record("fir", "edges/%s/%s" % (case, mix), group=case.split("/")[0], rms=r, max=m)
+    assert r <= FIR_RMS and m <= FIR_MAX, (case, mix, ra, ma, rb, mb, pb)
+
+
+@pytest.mark.parametrize("B,P", [(F2, 2), (F2, 3), (F4, 2), (F4, 3)])
+def test_fir_cluster_form_falls_back_on_misaligned_device_buffers(gpu_lib, B, P):
+    """run_device on torch buffers: whole blocks on 16-byte aligned rows take the cluster form; one whole block and
+    two ragged calls on buffers offset by one double (8-byte aligned) take the per-channel form, the stash and the head
+    kernel, which touch the caller's rows with 8-byte accesses only; the stream stays exact.  (A chain holding only this
+    FIR: the resampler stores double2 into the caller's output and does not fall back.)"""
+    import torch
+    C, T = 8, (P - 1) * B + 1
+    rng = np.random.default_rng(B + P)
+    h = ir_family("comb", T, C, seed=P)
+    nblk = 2 * P + 6
+    N = nblk * B
+    x = dyadic_signal(rng, N, C)
+    want = exact_conv(x, h, H_SHIFT)
+    ch = gpu_lib.Chain(48000, C).add_fir(h, block_hint=B)
+    st = torch.cuda.current_stream().cuda_stream
+    d_x = torch.from_numpy(x.reshape(-1)).cuda()
+    d_y = torch.zeros_like(d_x)
+    odd_x = torch.zeros(2 * B * C + 1, dtype=torch.float64, device="cuda")
+    odd_y = torch.zeros_like(odd_x)
+    # (frames, misaligned) per call: aligned blocks, one misaligned block, aligned, two misaligned ragged calls, aligned
+    calls = [(B, False)] * 3 + [(B, True)] + [(B, False)] * 2 + [(B // 2 - 3, True), (B // 2 + 3, True)]
+    calls += [(B, False)] * (nblk - 7)
+    pos = 0
+    for f, odd in calls:
+        a, b = pos * C, (pos + f) * C
+        if odd:
+            odd_x[1:1 + b - a] = d_x[a:b]
+            assert (odd_x.data_ptr() + 8) % 16 == 8
+            n = ch.run_device(0, f, odd_x.data_ptr() + 8, odd_y.data_ptr() + 8, st)
+            d_y[a:b] = odd_y[1:1 + b - a]
+        else:
+            assert (d_x.data_ptr() + 8 * a) % 16 == 0
+            n = ch.run_device(0, f, d_x.data_ptr() + 8 * a, d_y.data_ptr() + 8 * a, st)
+        assert n == f
+        pos += f
+    torch.cuda.synchronize()
+    got = d_y.cpu().numpy().reshape(N, C)
+    p = ch.describe()[0]
+    ch.close()
+    _check_plan(p, _fir_plan([(B, P)], tail_pf=2 if P == 3 else 0), "misaligned")
+    assert p["paths"] == dict(fused=1, cluster=nblk - 2, pipe=0, bulk=0, general=1, head=2), p["paths"]
+    r, m = fir_nerr(got, want, x, h)
+    _record("fir", "edges/misaligned/B%d_P%d" % (B, P), group="cluster", rms=r, max=m)
+    assert r <= FIR_RMS and m <= FIR_MAX, (B, P, r, m)
+
+
+@pytest.mark.parametrize("taps", [65, 20000])
+def test_fir_replans_twice_then_keeps_its_plan(gpu_lib, taps):
+    """No block hint: calls of 7, 150 and 300 frames plan B0 = 64, then re-plan to 128 and 256 (the kept input is
+    replayed through each new plan); after the second re-plan the plan stays, through a 9000-frame call and through
+    reset() with whole blocks and then ragged calls of up to 5000 frames."""
+    C = 3
+    steps = [(7, 64, 0), (150, 128, 1), (300, 256, 2), (9000, 256, 2)]
+    plans = {65: {64: [(64, 2)], 128: [(128, 1)], 256: [(256, 1)]},
+             20000: {B: _ladder(B, 4) for B in (64, 128, 256)}}[taps]
+    rng = np.random.default_rng(taps)
+    h = ir_family("flat", taps, C, seed=1)
+    N = max(11 * 4096, 16 * 256) + 77
+    x = dyadic_signal(rng, N, C)
+    want = exact_conv(x, h, H_SHIFT)
+    ch = gpu_lib.Chain(48000, C).add_fir(h)
+    outs, pos = [], 0
+    for f, B0, replans in steps:
+        outs.append(ch.run(x[pos:pos + f]).copy())
+        pos += f
+        p = ch.describe()[0]
+        assert [(L["B"], L["P"]) for L in p["levels"]] == plans[B0] and p["replans"] == replans, (f, p)
+        assert p["tail_pf"] == (1 if taps == 20000 else 0), p
+    sizes = []
+    while pos + sum(sizes) < N:
+        sizes.append(min(int(rng.integers(1, 2000)), N - pos - sum(sizes)))
+    got = np.concatenate(outs + [_run_sizes(ch, x[pos:], sizes)])
+    worst = [fir_nerr(got, want, x, h)]
+    ch.reset()
+    NA = N // 256 * 256
+    worst.append(fir_nerr(_run_sizes(ch, x[:NA], [256] * (NA // 256)), want[:NA], x[:NA], h))
+    ch.reset()
+    worst.append(fir_nerr(_run_sizes(ch, x, _ragged_sizes(rng, N, 256, lead=(600, 1, 5000))), want, x, h))
+    p = ch.describe()[0]
+    ch.close()
+    assert [(L["B"], L["P"]) for L in p["levels"]] == plans[256] and p["replans"] == 2, p
+    r, m = max(w[0] for w in worst), max(w[1] for w in worst)
+    _record("fir", "edges/replan/T%d" % taps, group="replan", rms=r, max=m)
+    assert r <= FIR_RMS and m <= FIR_MAX, (taps, worst)
 
 
 # ------------------------------------------------------------------------------------------------------------
