@@ -22,7 +22,8 @@
 //   k_fir_level0<B,P>   ONE kernel per level and block: forward transform, spectrum into the FDL, the first
 //                       pf = P partitions of S_j from registers, + Y_j (below), inverse transform, overlap.
 //                       On single-level plans it reads the caller's interleaved block and writes the caller's
-//                       result itself (clusters of four adjacent channels share the rows through DSMEM).
+//                       result itself (clusters of four adjacent channels share the rows through DSMEM); with a
+//                       batch tier it sums partitions 0 .. T+1 itself and starts from V_j ("folded": no k_fir_mac).
 //   k_fir_mac           Y_j = V_j + sum_{pf<=p<pf+T} X_{j-p} . H_p on a side stream, a block period ahead (the
 //                       blocks it needs were complete pf periods ago): the HBM-streaming kernel
 //   k_fir_mac_batch<T>  V_j = sum_{p>=pf+T} X_{j-p} . H_p for T periods at once (filter rows slide through a
@@ -32,7 +33,8 @@
 //   k_fir_stash/unstash interleaved <-> per-channel copies for multi-level plans and ragged calls
 // Spectra are stored "packed": B complex per row, bin 0 = (DC.re, Nyquist.re); rows are 16 B bytes
 // long, 128-byte aligned.  131072 taps, 4096-frame blocks: 1040 algorithmic bytes per sample for the plain
-// uniform scheme, 508 with the fused kernel + time-batched tail.
+// uniform scheme, 508 with the fused kernel + per-block MAC + time-batched tail, 476 with the per-block MAC folded
+// into the fused kernel.
 //
 // Calls that are not whole aligned blocks take the general path, exact for ANY frames-per-call
 // pattern: with R_j = sum_{1<=p<P0} X_{j-p} . H_p (completed level-0 blocks only)
@@ -273,7 +275,7 @@ struct L0Args {
 	int fdl_rows;            // rows per channel (slot arithmetic)
 	const double2 *H;        // [s or 0][rows][N]
 	long h_ch_stride;
-	int P, slot;
+	int P, slot;             // P: partitions summed (1, 2: compiled in; more: the folded tail, k_fir_level0<N, 0>)
 	double *out;             // [s][out_ch_stride]: first half + carry
 	long out_ch_stride;
 	double *carry;           // [s][N]
@@ -390,6 +392,8 @@ __device__ __forceinline__ double2 cmac(double2 acc, double2 x, double2 h)
 #ifndef FIR_L0_MAXNREG
 #define FIR_L0_MAXNREG 128
 #endif
+// P: partitions summed, or 0: a.P of them (single-level plans with a batch tier: the "folded" tail, partitions
+// 0 .. T+1, so that no per-block MAC and no Y spectrum round trip are needed)
 template <int N, int P, bool CL = false>
 __global__ void __launch_bounds__(FftCfg<N>::THREADS) __maxnreg__((N == 4096) ? FIR_L0_MAXNREG : 128) k_fir_level0(L0Args a)
 {
@@ -512,15 +516,23 @@ __global__ void __launch_bounds__(FftCfg<N>::THREADS) __maxnreg__((N == 4096) ? 
 		// arrives while the first transform runs (the CTA's warps all sit in the same phase, nothing else hides it).
 		// After the barrier: its release fence would wait for these requests too.
 		const double2 *Hc = a.H + (long) s * a.h_ch_stride;
-		prefetch_rows(Hc, (long) P * N * sizeof(double2), t, T);
-		const double2 *fc_ = a.fdl + (long) s * a.fdl_ch_stride;
+		if constexpr (P > 0) {
+			const double2 *fc_ = a.fdl + (long) s * a.fdl_ch_stride;
+			prefetch_rows(Hc, (long) P * N * sizeof(double2), t, T);
 #pragma unroll
-		for (int p = 1; p < P; ++p) {
-			const int sl = (a.slot - p < 0) ? a.slot - p + a.fdl_rows : a.slot - p;
-			prefetch_rows(fc_ + (long) sl * N, (long) N * sizeof(double2), t, T);
+			for (int p = 1; p < P; ++p) {
+				const int sl = (a.slot - p < 0) ? a.slot - p + a.fdl_rows : a.slot - p;
+				prefetch_rows(fc_ + (long) sl * N, (long) N * sizeof(double2), t, T);
+			}
+			prefetch_rows(a.carry + (long) s * N, (long) N * sizeof(double), t, T);
+			if (a.init) prefetch_rows(a.init + (long) s * N, (long) N * sizeof(double2), t, T);
 		}
-		prefetch_rows(a.carry + (long) s * N, (long) N * sizeof(double), t, T);
-		if (a.init) prefetch_rows(a.init + (long) s * N, (long) N * sizeof(double2), t, T);
+		else {
+			// The folded tail reads 2 a.P rows and more per channel, and one wave of CTAs sums them in step: rows pulled
+			// ahead evict the rows being summed (measured: a prefetch of partitions 0 and 1 here and of partition p+1
+			// during partition p made the step 17% slower than this).  Only H_0, read right after the transform.
+			prefetch_rows(Hc, (long) N * sizeof(double2), t, T);
+		}
 	}
 	fft_forward_smem<N>(buf, a.ptw, t);
 	if (active) {
@@ -577,8 +589,7 @@ __global__ void __launch_bounds__(FftCfg<N>::THREADS) __maxnreg__((N == 4096) ? 
 				buf[spad(n)] = cmul(xn, hn[i]);
 			}
 		}
-#pragma unroll
-		for (int p = 1; p < P; ++p) {
+		auto mac_partition = [&](int p) {
 			const int sl = (a.slot - p < 0) ? a.slot - p + a.fdl_rows : a.slot - p;
 			const double2 *Xp = fdl + (long) sl * N, *Hp = H + (long) p * N;
 #pragma unroll
@@ -602,11 +613,20 @@ __global__ void __launch_bounds__(FftCfg<N>::THREADS) __maxnreg__((N == 4096) ? 
 					buf[spad(n)] = cmac(buf[spad(n)], xn[i], hn[i]);
 				}
 			}
+		};
+		if constexpr (P > 0) {
+#pragma unroll
+			for (int p = 1; p < P; ++p) mac_partition(p);
+		}
+		else {
+#pragma unroll 1
+			for (int p = 1; p < a.P; ++p) mac_partition(p);
 		}
 #pragma unroll
 		for (int half = 0; half < 8; half += 4) {
-			// what the other partitions of this level contribute (MAC kernels, a block period ahead): summed here, in
-			// the frequency domain, so that the level needs one inverse transform
+			// what the other partitions of this level contribute (`init`: Y_j of the per-block MAC, or the batch tier's
+			// V_j when this kernel sums the near partitions itself): summed here, in the frequency domain, so that the
+			// level needs one inverse transform
 			double2 yk[4], yn[4], w2[4];
 #pragma unroll
 			for (int i = 0; i < 4; ++i) {
@@ -1182,9 +1202,11 @@ static int configure_n()
 		CUDA_TRY(cudaFuncSetAttribute(k_fir_inv<N>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int) FftCfg<N>::SMEM), return -1);
 		CUDA_TRY(cudaFuncSetAttribute((k_fir_level0<N, 1>), cudaFuncAttributeMaxDynamicSharedMemorySize, (int) level0_smem<N>()), return -1);
 		CUDA_TRY(cudaFuncSetAttribute((k_fir_level0<N, 2>), cudaFuncAttributeMaxDynamicSharedMemorySize, (int) level0_smem<N>()), return -1);
+		CUDA_TRY(cudaFuncSetAttribute((k_fir_level0<N, 0>), cudaFuncAttributeMaxDynamicSharedMemorySize, (int) level0_smem<N>()), return -1);
 		if constexpr (FftCfg<N>::CPB <= 2) {
 			CUDA_TRY(cudaFuncSetAttribute((k_fir_level0<N, 1, true>), cudaFuncAttributeMaxDynamicSharedMemorySize, (int) level0_smem<N>(true)), return -1);
 			CUDA_TRY(cudaFuncSetAttribute((k_fir_level0<N, 2, true>), cudaFuncAttributeMaxDynamicSharedMemorySize, (int) level0_smem<N>(true)), return -1);
+			CUDA_TRY(cudaFuncSetAttribute((k_fir_level0<N, 0, true>), cudaFuncAttributeMaxDynamicSharedMemorySize, (int) level0_smem<N>(true)), return -1);
 		}
 		configured[dev & 63].store(1);
 	}
@@ -1227,13 +1249,15 @@ static int launch_level0_n(const L0Args &a, cudaStream_t st)
 			attr.val.clusterDim.x = 4 / CPB; attr.val.clusterDim.y = 1; attr.val.clusterDim.z = 1;
 			cfg.attrs = &attr; cfg.numAttrs = 1;
 			if (a.P == 1) CUDA_TRY(cudaLaunchKernelEx(&cfg, k_fir_level0<N, 1, true>, a), return -1);
-			else CUDA_TRY(cudaLaunchKernelEx(&cfg, k_fir_level0<N, 2, true>, a), return -1);
+			else if (a.P == 2) CUDA_TRY(cudaLaunchKernelEx(&cfg, k_fir_level0<N, 2, true>, a), return -1);
+			else CUDA_TRY(cudaLaunchKernelEx(&cfg, k_fir_level0<N, 0, true>, a), return -1);
 			g_kernel_launches.fetch_add(1, std::memory_order_relaxed);
 			return 0;
 		}
 	}
 	if (a.P == 1) LAUNCH((k_fir_level0<N, 1>), ceil_div(a.n_ch, FftCfg<N>::CPB), FftCfg<N>::THREADS, level0_smem<N>(), st, a);
-	else LAUNCH((k_fir_level0<N, 2>), ceil_div(a.n_ch, FftCfg<N>::CPB), FftCfg<N>::THREADS, level0_smem<N>(), st, a);
+	else if (a.P == 2) LAUNCH((k_fir_level0<N, 2>), ceil_div(a.n_ch, FftCfg<N>::CPB), FftCfg<N>::THREADS, level0_smem<N>(), st, a);
+	else LAUNCH((k_fir_level0<N, 0>), ceil_div(a.n_ch, FftCfg<N>::CPB), FftCfg<N>::THREADS, level0_smem<N>(), st, a);
 	return 0;
 }
 
@@ -1419,6 +1443,10 @@ struct FirOp : Op {
 	cudaEvent_t ev_bs[8] = {};           // after the tier launches of a block (ring), ev_bs_last: the latest one
 	int ev_bs_n = 0;
 	cudaEvent_t ev_bs_last = nullptr;
+	// folded tail: the fused kernel of block j starts from V_j, which the tier launches up to block j-3 complete;
+	// ev_bs_at[q & 3] = ev_bs_last as it was after block q
+	bool fold = false;
+	cudaEvent_t ev_bs_at[4] = {};
 	cudaEvent_t ev_join[2] = { nullptr, nullptr };
 	// single-level tail plans: the fused kernel of every block goes to a stream of the highest priority (the caller's
 	// stream hands over and takes back with two events): its CTAs are placed before the queued CTAs of the
@@ -1443,6 +1471,9 @@ struct FirOp : Op {
 
 	const char *name() const override { return "fir"; }
 
+	// partitions level 0's fused kernel sums on whole aligned blocks
+	int l0_parts() const { return fold ? t_batch + 2 : (lv[0].P < 2) ? lv[0].P : 2; }
+
 	std::string describe() const override
 	{
 		char buf[1024];
@@ -1450,8 +1481,8 @@ struct FirOp : Op {
 		                 filter_frames, n_sel, fc, latency, planned ? 1 : 0);
 		for (int l = 0; l < n_levels && n < (int) sizeof(buf) - 64; ++l)
 			n += snprintf(buf + n, sizeof(buf) - n, "%s{\"B\":%d,\"P\":%d}", l ? "," : "", lv[l].B, lv[l].P);
-		n += snprintf(buf + n, sizeof(buf) - n, "],\"t_batch\":%d,\"t_far\":%d,\"far_e\":%d,\"far_classes\":%d,\"stagger\":%d,\"merge\":%d,\"tail_pf\":%d,\"bulk\":%d,\"pipe\":%d,\"pipe_pf\":%d,",
-		              t_batch, t_far, far_e, far_classes, stagger ? 1 : 0, merge_tail ? 1 : 0, tail_pf, nb_max, use_pipe ? 1 : 0, pipe_pf);
+		n += snprintf(buf + n, sizeof(buf) - n, "],\"t_batch\":%d,\"t_far\":%d,\"far_e\":%d,\"far_classes\":%d,\"stagger\":%d,\"merge\":%d,\"tail_pf\":%d,\"l0_parts\":%d,\"bulk\":%d,\"pipe\":%d,\"pipe_pf\":%d,",
+		              t_batch, t_far, far_e, far_classes, stagger ? 1 : 0, merge_tail ? 1 : 0, tail_pf, l0_parts(), nb_max, use_pipe ? 1 : 0, pipe_pf);
 		snprintf(buf + n, sizeof(buf) - n, "\"replans\":%d,\"paths\":{\"fused\":%ld,\"cluster\":%ld,\"pipe\":%ld,\"bulk\":%ld,\"general\":%ld,\"head\":%ld}}",
 		         replans, n_fused, n_cluster, n_pipe, n_bulk, n_general, n_head);
 		return buf;
@@ -1481,6 +1512,8 @@ struct FirOp : Op {
 		for (cudaEvent_t &e : ev_batch) { if (e) cudaEventDestroy(e); e = nullptr; }
 		for (cudaEvent_t &e : ev_bs) { if (e) cudaEventDestroy(e); e = nullptr; }
 		ev_bs_last = nullptr; ev_bs_n = 0;
+		for (cudaEvent_t &e : ev_bs_at) e = nullptr;
+		fold = false;
 		for (cudaEvent_t &e : ev_tail) { if (e) cudaEventDestroy(e); e = nullptr; }
 		for (cudaEvent_t &e : ev_join) { if (e) cudaEventDestroy(e); e = nullptr; }
 		if (ev_main) cudaEventDestroy(ev_main);
@@ -1577,8 +1610,6 @@ struct FirOp : Op {
 				CUDA_TRY(cudaStreamCreateWithPriority(&side, cudaStreamNonBlocking, side_prio), return -1);
 				CUDA_TRY(cudaEventCreateWithFlags(&ev_main, cudaEventDisableTiming), return -1);
 				CUDA_TRY(cudaEventCreateWithFlags(&ev_urgent, cudaEventDisableTiming), return -1);
-				CUDA_TRY(cudaEventCreateWithFlags(&ev_tail[0], cudaEventDisableTiming), return -1);
-				CUDA_TRY(cudaEventCreateWithFlags(&ev_tail[1], cudaEventDisableTiming), return -1);
 			}
 			if (has_tail) {
 				L.tail = true;
@@ -1587,10 +1618,6 @@ struct FirOp : Op {
 				// headline (DESIGN.md K2), it stays selectable for measurements and is covered by the tests
 				const char *pe = getenv("DSP_B200_FIR_PIPE");
 				use_pipe = (l == 0) && direct_io && pipe_size_ok(L.B) && (pe && pe[0] == '1');
-				if (!use_pipe) {
-					d_Y_side = dev_alloc<double2>((size_t) pf * n_sel * L.B);
-					if (!d_Y_side) return -1;
-				}
 				const char *he = getenv("DSP_B200_FIR_HOT");
 				if (!use_pipe && l == 0 && direct_io && !(he && he[0] == '0')) {
 					int lo = 0, hi = 0;
@@ -1651,6 +1678,24 @@ struct FirOp : Op {
 				if (use_pipe) {
 					pipe_pf = (t_batch > 0) ? t_batch + 2 : L.P;
 					if (getenv("DSP_B200_FIR_PIPE_STATS")) d_stats = dev_alloc<long long>(8 * 1024);
+				}
+				// Folded tail (single level, direct I/O, a batch tier): the fused kernel sums partitions 0 .. t_batch+1 and
+				// starts from the near tier's V_j -- no per-block MAC, no Y spectrum through HBM (476 instead of 508 bytes
+				// per sample on the headline, DESIGN.md K2).  Only when the fused kernel's CTAs outnumber half the SMs: with
+				// fewer, the per-block MAC streams on the SMs the fused kernel leaves idle, and moving its partitions into
+				// the few fused CTAs lengthens the step (64 channels of 4096 frames: 8% slower folded, 256: 6% faster).
+				// DSP_B200_FIR_FOLD=1 / 0 force either form (tests, measurements); the merged grid is a per-block MAC.
+				const char *fe = getenv("DSP_B200_FIR_FOLD");
+				const int cpb = (L.B / 16 >= 256) ? 1 : 256 / (L.B / 16);   // FftCfg<B>::CPB
+				const bool fold_pays = 2 * ceil_div(n_sel, cpb) > sm_count();
+				fold = l == 0 && !use_pipe && direct_io && t_batch > 0 && !merge_tail && (fe ? fe[0] == '1' : fold_pays);
+				if (!use_pipe && !fold) {
+					d_Y_side = dev_alloc<double2>((size_t) pf * n_sel * L.B);
+					if (!d_Y_side) return -1;
+					if (l == 0) {
+						CUDA_TRY(cudaEventCreateWithFlags(&ev_tail[0], cudaEventDisableTiming), return -1);
+						CUDA_TRY(cudaEventCreateWithFlags(&ev_tail[1], cudaEventDisableTiming), return -1);
+					}
 				}
 			}
 			if (L.B > Bmax) Bmax = L.B;
@@ -1731,6 +1776,7 @@ struct FirOp : Op {
 		if (d_V) cudaMemsetAsync(d_V, 0, (size_t) 2 * t_batch * n_sel * lv[n_levels - 1].B * sizeof(double2), st);
 		if (d_V2) cudaMemsetAsync(d_V2, 0, (size_t) 2 * t_far * n_sel * lv[n_levels - 1].B * sizeof(double2), st);
 		ev_bs_last = nullptr;
+		for (cudaEvent_t &e : ev_bs_at) e = nullptr;
 		for (int l = 0; l < n_levels; ++l) {
 			FirLevel &L = lv[l];
 			L.blk = 0;
@@ -1875,6 +1921,13 @@ struct FirOp : Op {
 			}
 			return 0;
 		}
+		if (fold) {
+			// no per-block MAC: the fused kernel of block j sums partitions 2 .. t_batch+1 itself
+			if (!serial) CUDA_TRY(cudaEventRecord(ev_main, st), return -1);
+			if (launch_tiers0(L, q, bs, serial)) return -1;
+			ev_bs_at[q & 3] = ev_bs_last;
+			return 0;
+		}
 		double2 *Y = d_Y_side + (size_t) (j & 1) * n_sel * L.B;
 		if (!serial) {
 			CUDA_TRY(cudaEventRecord(ev_main, st), return -1);
@@ -1963,7 +2016,8 @@ struct FirOp : Op {
 
 	// The main stream may only go on with block `blk` of a single-level tail plan once the tier launches that read FDL
 	// row blk % P (those after the blocks up to blk-4) are complete.  The fused kernel's path gets that from waiting
-	// for Y_blk (whose MAC waited for the launches up to blk-3); the general path waits here, for all of them.
+	// for Y_blk (whose MAC waited for the launches up to blk-3) or, folded, for the launches up to blk-3 themselves;
+	// the general path waits here, for all of them.
 	int wait_batch_for(long blk, cudaStream_t st)
 	{
 		(void) blk;
@@ -2200,7 +2254,7 @@ struct FirOp : Op {
 					}
 					f.fdl = L0.fdl; f.fdl_ch_stride = (long) L0.R * B0; f.fdl_rows = L0.R;
 					f.H = L0.H; f.h_ch_stride = (fc == 1) ? 0 : (long) L0.P * B0;
-					f.P = (L0.P < 2) ? L0.P : 2; f.slot = (int) (L0.blk % L0.R);
+					f.P = l0_parts(); f.slot = (int) (L0.blk % L0.R);
 					f.out = d_ytmp; f.out_ch_stride = B0; f.carry = L0.carry; f.tw = L0.tw; f.ptw = L0.ptw; f.n_ch = n_sel;
 					cudaStream_t ls = st;
 					// (not in a synchronous host call: it works on one block at a time, the two event hops cost it time per
@@ -2211,7 +2265,16 @@ struct FirOp : Op {
 						CUDA_TRY(cudaStreamWaitEvent(hot, ev_hot_in, 0), return -1);
 						ls = hot;
 					}
-					if (tail_pf == 2 && L0.blk >= 2) {
+					if (fold) {
+						// V_j: complete once the tier launches up to block j-3 are, and nothing overwrites its slot before
+						// block j+2's launch; those launches have read FDL row j % P (blocks up to j-4 read it) as well.
+						// Before block 3 no launch has covered V_j: it is zero (the blocks it sums do not exist).
+						if (L0.blk >= 3) {
+							if (cudaEvent_t e = ev_bs_at[(L0.blk - 3) & 3]) CUDA_TRY(cudaStreamWaitEvent(ls, e, 0), return -1);
+							f.init = d_V + (size_t) (L0.blk % (2 * t_batch)) * n_sel * B0;
+						}
+					}
+					else if (tail_pf == 2 && L0.blk >= 2) {
 						// Y of this block was launched two blocks ago (advance_tail0)
 						CUDA_TRY(cudaStreamWaitEvent(ls, ev_tail[L0.blk & 1], 0), return -1);
 						f.init = d_Y_side + (size_t) (L0.blk & 1) * n_sel * B0;
