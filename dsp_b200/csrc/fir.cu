@@ -23,18 +23,20 @@
 //                       pf = P partitions of S_j from registers, + Y_j (below), inverse transform, overlap.
 //                       On single-level plans it reads the caller's interleaved block and writes the caller's
 //                       result itself (clusters of four adjacent channels share the rows through DSMEM); with a
-//                       batch tier it sums partitions 0 .. T+1 itself and starts from V_j ("folded": no k_fir_mac).
+//                       batch tier it starts from V_j and sums the partitions the tier left out: 0 .. 2+t when V_j
+//                       came from the launch after block j-3-t ("folded": no k_fir_mac).
 //   k_fir_mac           Y_j = V_j + sum_{pf<=p<pf+T} X_{j-p} . H_p on a side stream, a block period ahead (the
 //                       blocks it needs were complete pf periods ago): the HBM-streaming kernel
 //   k_fir_mac_batch<T>  V_j = sum_{p>=pf+T} X_{j-p} . H_p for T periods at once (filter rows slide through a
-//                       register window: every FDL and filter row is read once per T outputs)
+//                       register window: every FDL and filter row is read once per T outputs); folded, the near
+//                       tier also takes every partition p < pf+T whose block is complete (the triangle p >= 3+t)
 //   k_fir_mac_bulk<8>   calls that bring several whole 8192-blocks: all partitions of up to 8 new blocks in
 //                       one pass, with one forward and one inverse launch (k_fir_fwd / k_fir_inv, gridDim.y)
 //   k_fir_stash/unstash interleaved <-> per-channel copies for multi-level plans and ragged calls
 // Spectra are stored "packed": B complex per row, bin 0 = (DC.re, Nyquist.re); rows are 16 B bytes
 // long, 128-byte aligned.  131072 taps, 4096-frame blocks: 1040 algorithmic bytes per sample for the plain
 // uniform scheme, 508 with the fused kernel + per-block MAC + time-batched tail, 476 with the per-block MAC folded
-// into the fused kernel.
+// into the fused kernel, 440 with the near tier taking the triangle of partitions its rows already meet.
 //
 // Calls that are not whole aligned blocks take the general path, exact for ANY frames-per-call
 // pattern: with R_j = sum_{1<=p<P0} X_{j-p} . H_p (completed level-0 blocks only)
@@ -276,6 +278,11 @@ struct L0Args {
 	const double2 *H;        // [s or 0][rows][N]
 	long h_ch_stride;
 	int P, slot;             // P: partitions summed (1, 2: compiled in; more: the folded tail, k_fir_level0<N, 0>)
+	// folded tail (cls_T > 0): block blk's V_j of channel s comes from the near-tier launch of its class
+	// c = (s / cls_w) % cls_K that covers j, made t = (blk - 3 - c) mod cls_T blocks earlier; it holds the partitions
+	// from 3 + t on, the kernel sums 0 .. 2 + t (all P while no launch has covered j)
+	long blk;
+	int cls_T, cls_K, cls_w;
 	double *out;             // [s][out_ch_stride]: first half + carry
 	long out_ch_stride;
 	double *carry;           // [s][N]
@@ -392,8 +399,9 @@ __device__ __forceinline__ double2 cmac(double2 acc, double2 x, double2 h)
 #ifndef FIR_L0_MAXNREG
 #define FIR_L0_MAXNREG 128
 #endif
-// P: partitions summed, or 0: a.P of them (single-level plans with a batch tier: the "folded" tail, partitions
-// 0 .. T+1, so that no per-block MAC and no Y spectrum round trip are needed)
+// P: partitions summed, or 0: a run-time count of at most a.P (single-level plans with a batch tier: the "folded" tail,
+// partitions 0 .. 2+t of a channel whose V_j came from the near-tier launch after block j-3-t, so that no per-block MAC
+// and no Y spectrum round trip are needed)
 template <int N, int P, bool CL = false>
 __global__ void __launch_bounds__(FftCfg<N>::THREADS) __maxnreg__((N == 4096) ? FIR_L0_MAXNREG : 128) k_fir_level0(L0Args a)
 {
@@ -619,8 +627,15 @@ __global__ void __launch_bounds__(FftCfg<N>::THREADS) __maxnreg__((N == 4096) ? 
 			for (int p = 1; p < P; ++p) mac_partition(p);
 		}
 		else {
+			// (d < 0: the class's first launch covers a later period.  The two transform groups of a 2048-point CTA may
+			// loop a different number of times: no barrier inside.)
+			int np = a.P;
+			if (a.cls_T > 0) {
+				const long d = a.blk - 3 - (s >> (__ffs(a.cls_w) - 1)) % a.cls_K;
+				if (d >= 0) np = 3 + (int) (d % a.cls_T);
+			}
 #pragma unroll 1
-			for (int p = 1; p < a.P; ++p) mac_partition(p);
+			for (int p = 1; p < np; ++p) mac_partition(p);
 		}
 #pragma unroll
 		for (int half = 0; half < 8; half += 4) {
@@ -832,15 +847,16 @@ __global__ void __launch_bounds__(256, FIR_MAC_MINB) k_fir_mac(MacArgs a)
 	else fir_mac_body<SHARED_H, false>(a, blockIdx.y);
 }
 
-// Time-batched tail of the last level.  With V_j = sum_{p in [p_lo, p_hi)} X_{j-p} H_p, p_lo >= pf+T (the part of
-// block period j's spectrum that only involves blocks at least pf+T periods old; pf = partitions summed inside the
-// fused FFT kernel), one launch after block q completes produces V_j for the T periods j = q+pf+1 .. q+pf+T at once:
-// every FDL row and every filter row is streamed ONCE for T outputs (the filter rows slide through a T-deep
-// register window), instead of once per output.
-// V_t[k] = Vin_t[k] + sum_m X_{q+pf+1-m}[k] * H_{m+t}[k] over the (m, t) with p_lo <= m+t < p_hi.
-// Tiers: a deeper batch (larger T) may only take older partitions (p >= pf+T) but reads the filter less often; the
-// plan stacks two of them -- the far tier's result is the near tier's starting value `Vin`, the near tier's result
-// is what the per-block MAC starts from.
+// Time-batched tail of the last level.  One launch after block q completes produces V_j for the T periods
+// j = q+pf+1 .. q+pf+T at once (pf = partitions summed inside the fused FFT kernel): every FDL row and every filter
+// row is streamed ONCE for T outputs (the filter rows slide through a T-deep register window), instead of once per
+// output.  V_t[k] = Vin_t[k] + sum_{m>pf} X_{q+pf+1-m}[k] * H_{m+t}[k] over the (m, t) with p_lo <= m+t < p_hi: only
+// blocks up to q.  With p_lo >= pf+T that is V_j = sum_{p in [p_lo, p_hi)} X_{j-p} H_p for every t (the per-block MAC
+// adds the same partitions to every period); with p_lo = pf+1 (the folded near tier) period t gets the partitions
+// p >= pf+1+t -- a triangle of partitions 0 .. pf+T-1 is left to the fused kernel, which sums 0 .. pf+t.
+// Tiers: a deeper batch (larger T) reads the filter less often; the plan stacks two of them -- the far tier's result
+// is the near tier's starting value `Vin`, the near tier's result is what the per-block MAC or the fused kernel starts
+// from.
 struct MacBatchArgs {
 	const double2 *fdl;   // [s][P][N]
 	const double2 *H;     // [s][P][N] or [P][N]
@@ -850,7 +866,9 @@ struct MacBatchArgs {
 	int n_slots;
 	long h_ch_stride;
 	int pf;               // partitions 0..pf-1 are summed by the level's fused FFT kernel (1: upper levels, 2: level 0)
-	int s_first, s_step;  // channel of blockIdx.y: s_first + blockIdx.y * s_step (0, 1: all channels)
+	// channels of this launch: class g of K, the classes taking turns over groups of w adjacent channels; blockIdx.y = y
+	// is channel (g + K (y / w)) w + y % w (0, 1, 1: all channels)
+	int g, K, w;
 	int p_lo, p_hi;       // partitions of this tier
 	const double2 *Vin;   // [slot][s][N], slot = j mod vin_slots: a farther tier's sums to start from (NULL: zero)
 	int vin_slots;
@@ -875,22 +893,22 @@ template <int T, bool SHARED_H, bool DCW>
 __device__ __forceinline__ void fir_mac_batch_body(const MacBatchArgs &a, int y)
 {
 	const int k = blockIdx.x * blockDim.x + threadIdx.x;
-	const int s = a.s_first + y * a.s_step;
+	const int wl = __ffs(a.w) - 1;   // w: a power of two
+	const int s = ((a.g + a.K * (y >> wl)) << wl) + (y & (a.w - 1));
 	const double2 *fdl = a.fdl + (long) s * a.P * a.N + k;
 	const double2 *H = a.H + (long) s * a.h_ch_stride + k;
 	const bool dc = DCW && (k == 0);
 	const double2 zero = make_double2(0.0, 0.0);
 	double2 acc[T], hw[T];
 #define HROW(p) (((p) >= a.p_lo && (p) < a.p_hi) ? (SHARED_H ? __ldg(&H[(long) (p) * a.N]) : __ldcs(&H[(long) (p) * a.N])) : zero)
-	int m = a.p_lo - T + 1;   // first row that meets a partition of this tier: X_{q+pf+1-m} (m >= pf+1: it exists)
+	int m = a.pf + 1;   // first row: the newest complete block, X_q
 #pragma unroll
 	for (int t = 0; t < T; ++t) {
 		const long j = a.q + a.pf + 1 + t;
 		acc[t] = a.Vin ? __ldcs(&a.Vin[((j % a.vin_slots) * a.n_sel + s) * (long) a.N + k]) : zero;
 		hw[t] = HROW(m + t);
 	}
-	int slot = (int) ((a.q + a.pf + 1 - m) % a.P);   // row of X_{q+pf+1-m}
-	if (slot < 0) slot += a.P;
+	int slot = (int) (a.q % a.P);   // row of X_{q+pf+1-m} = X_q
 #define XROW(d) __ldcs(&fdl[(long) ((slot - (d) < 0) ? slot - (d) + a.P : slot - (d)) * a.N])
 #define STEP(XV, HN)                                                          \
 	do {                                                                      \
@@ -1447,6 +1465,9 @@ struct FirOp : Op {
 	// ev_bs_at[q & 3] = ev_bs_last as it was after block q
 	bool fold = false;
 	cudaEvent_t ev_bs_at[4] = {};
+	// staggered folded plans: the classes take turns over groups of class_w adjacent channels (1 otherwise), so that
+	// the four channels of a cluster sum the same number of partitions and finish together
+	int class_w = 1;
 	cudaEvent_t ev_join[2] = { nullptr, nullptr };
 	// single-level tail plans: the fused kernel of every block goes to a stream of the highest priority (the caller's
 	// stream hands over and takes back with two events): its CTAs are placed before the queued CTAs of the
@@ -1471,8 +1492,10 @@ struct FirOp : Op {
 
 	const char *name() const override { return "fir"; }
 
-	// partitions level 0's fused kernel sums on whole aligned blocks
+	// partitions level 0's fused kernel sums on whole aligned blocks: at most, and (folded: once every class has had a
+	// near-tier launch) at least
 	int l0_parts() const { return fold ? t_batch + 2 : (lv[0].P < 2) ? lv[0].P : 2; }
+	int l0_parts_min() const { return fold ? 3 : l0_parts(); }
 
 	std::string describe() const override
 	{
@@ -1481,8 +1504,10 @@ struct FirOp : Op {
 		                 filter_frames, n_sel, fc, latency, planned ? 1 : 0);
 		for (int l = 0; l < n_levels && n < (int) sizeof(buf) - 64; ++l)
 			n += snprintf(buf + n, sizeof(buf) - n, "%s{\"B\":%d,\"P\":%d}", l ? "," : "", lv[l].B, lv[l].P);
-		n += snprintf(buf + n, sizeof(buf) - n, "],\"t_batch\":%d,\"t_far\":%d,\"far_e\":%d,\"far_classes\":%d,\"stagger\":%d,\"merge\":%d,\"tail_pf\":%d,\"l0_parts\":%d,\"bulk\":%d,\"pipe\":%d,\"pipe_pf\":%d,",
-		              t_batch, t_far, far_e, far_classes, stagger ? 1 : 0, merge_tail ? 1 : 0, tail_pf, l0_parts(), nb_max, use_pipe ? 1 : 0, pipe_pf);
+		n += snprintf(buf + n, sizeof(buf) - n, "],\"t_batch\":%d,\"t_far\":%d,\"far_e\":%d,\"far_classes\":%d,\"stagger\":%d,\"class_width\":%d,\"merge\":%d,\"tail_pf\":%d,"
+		              "\"l0_parts\":%d,\"l0_parts_min\":%d,\"bulk\":%d,\"pipe\":%d,\"pipe_pf\":%d,",
+		              t_batch, t_far, far_e, far_classes, stagger ? 1 : 0, class_w, merge_tail ? 1 : 0, tail_pf, l0_parts(), l0_parts_min(), nb_max,
+		              use_pipe ? 1 : 0, pipe_pf);
 		snprintf(buf + n, sizeof(buf) - n, "\"replans\":%d,\"paths\":{\"fused\":%ld,\"cluster\":%ld,\"pipe\":%ld,\"bulk\":%ld,\"general\":%ld,\"head\":%ld}}",
 		         replans, n_fused, n_cluster, n_pipe, n_bulk, n_general, n_head);
 		return buf;
@@ -1514,6 +1539,7 @@ struct FirOp : Op {
 		ev_bs_last = nullptr; ev_bs_n = 0;
 		for (cudaEvent_t &e : ev_bs_at) e = nullptr;
 		fold = false;
+		class_w = 1;
 		for (cudaEvent_t &e : ev_tail) { if (e) cudaEventDestroy(e); e = nullptr; }
 		for (cudaEvent_t &e : ev_join) { if (e) cudaEventDestroy(e); e = nullptr; }
 		if (ev_main) cudaEventDestroy(ev_main);
@@ -1679,16 +1705,24 @@ struct FirOp : Op {
 					pipe_pf = (t_batch > 0) ? t_batch + 2 : L.P;
 					if (getenv("DSP_B200_FIR_PIPE_STATS")) d_stats = dev_alloc<long long>(8 * 1024);
 				}
-				// Folded tail (single level, direct I/O, a batch tier): the fused kernel sums partitions 0 .. t_batch+1 and
-				// starts from the near tier's V_j -- no per-block MAC, no Y spectrum through HBM (476 instead of 508 bytes
-				// per sample on the headline, DESIGN.md K2).  Only when the fused kernel's CTAs outnumber half the SMs: with
-				// fewer, the per-block MAC streams on the SMs the fused kernel leaves idle, and moving its partitions into
-				// the few fused CTAs lengthens the step (64 channels of 4096 frames: 8% slower folded, 256: 6% faster).
+				// Folded tail (single level, direct I/O, a batch tier): the fused kernel starts from the near tier's V_j and
+				// sums what that tier leaves out, 3 .. t_batch+2 partitions (launch_tiers0) -- no per-block MAC, no Y spectrum
+				// through HBM (440 instead of 508 bytes per sample on the headline, DESIGN.md K2).  Only when the fused
+				// kernel's CTAs outnumber half the SMs: with fewer, the per-block MAC streams on the SMs the fused kernel
+				// leaves idle, and moving its partitions into the few fused CTAs lengthens the step (64 channels of 4096
+				// frames: 8% slower folded, 256: 6% faster).
 				// DSP_B200_FIR_FOLD=1 / 0 force either form (tests, measurements); the merged grid is a per-block MAC.
 				const char *fe = getenv("DSP_B200_FIR_FOLD");
 				const int cpb = (L.B / 16 >= 256) ? 1 : 256 / (L.B / 16);   // FftCfg<B>::CPB
 				const bool fold_pays = 2 * ceil_div(n_sel, cpb) > sm_count();
 				fold = l == 0 && !use_pipe && direct_io && t_batch > 0 && !merge_tail && (fe ? fe[0] == '1' : fold_pays);
+				// staggered classes of up to 4 adjacent channels (a cluster's four when there are enough channels for every
+				// class to have a whole group): all CTAs of a cluster sum the same partitions, and a cluster that finishes
+				// early hands its SMs to the queued batch CTAs at once instead of waiting for its slowest channel
+				if (fold && stagger) {
+					const int most = (n_sel / t_batch < 4) ? n_sel / t_batch : 4;
+					while (class_w * 2 <= most) class_w *= 2;
+				}
 				if (!use_pipe && !fold) {
 					d_Y_side = dev_alloc<double2>((size_t) pf * n_sel * L.B);
 					if (!d_Y_side) return -1;
@@ -1876,7 +1910,7 @@ struct FirOp : Op {
 				b.h_ch_stride = (fc == 1) ? 0 : (long) L.P * L.B;
 				b.pf = 1;
 				b.p_lo = t_batch + 1; b.p_hi = L.P;
-				b.s_first = 0; b.s_step = 1;
+				b.g = 0; b.K = 1; b.w = 1;
 				const int threads = (L.B < batch_threads_for(t_batch)) ? L.B : batch_threads_for(t_batch);
 				dim3 grid(L.B / threads, n_sel);
 				launch_mac_batch(t_batch, fc == 1, grid, threads, bs, b);
@@ -1913,7 +1947,7 @@ struct FirOp : Op {
 					b.h_ch_stride = (fc == 1) ? 0 : (long) L.P * L.B;
 					b.pf = 2;
 					b.p_lo = t_batch + 2; b.p_hi = L.P;
-					b.s_first = g; b.s_step = t_batch;
+					b.g = g; b.K = t_batch; b.w = 1;
 					const int threads = (L.B < batch_threads_for(t_batch)) ? L.B : batch_threads_for(t_batch);
 					dim3 grid(L.B / threads, (n_sel - g + t_batch - 1) / t_batch);
 					launch_mac_batch(t_batch, fc == 1, grid, threads, st, b);
@@ -1922,7 +1956,7 @@ struct FirOp : Op {
 			return 0;
 		}
 		if (fold) {
-			// no per-block MAC: the fused kernel of block j sums partitions 2 .. t_batch+1 itself
+			// no per-block MAC: the fused kernel of block j sums the partitions the near tier leaves to it
 			if (!serial) CUDA_TRY(cudaEventRecord(ev_main, st), return -1);
 			if (launch_tiers0(L, q, bs, serial)) return -1;
 			ev_bs_at[q & 3] = ev_bs_last;
@@ -1944,7 +1978,7 @@ struct FirOp : Op {
 			ta.b.fdl = L.fdl; ta.b.H = L.H; ta.b.N = L.B; ta.b.P = L.P; ta.b.n_sel = n_sel; ta.b.q = q;
 			ta.b.V = d_V; ta.b.n_slots = 2 * t_batch; ta.b.h_ch_stride = ta.m.h_ch_stride;
 			ta.b.pf = 2; ta.b.p_lo = t_batch + 2; ta.b.p_hi = L.P;
-			ta.b.s_first = g; ta.b.s_step = t_batch;
+			ta.b.g = g; ta.b.K = t_batch; ta.b.w = 1;
 			ta.n_batch_y = (n_sel > g) ? (n_sel - g + t_batch - 1) / t_batch : 0;
 			const dim3 grid(L.B / 256, ta.n_batch_y + n_sel);
 			{
@@ -1971,22 +2005,26 @@ struct FirOp : Op {
 
 	// Tier launches after block q of a single-level plan (far tier first: the near tier starts from its sums).  A tier
 	// of depth T produces V_j = (farther tier's V_j) + sum_{p in tier} X_{j-p} H_p for the T periods j = q+3 .. q+2+T
-	// from the blocks up to q.  Staggered: for the channels s with s mod T == q mod T, every block; otherwise for all
-	// channels when q mod T == 0.  Both ways a channel's periods j are covered exactly once, and the near tier's
-	// window of a channel lies inside one far window of that channel (t_far is a multiple of t_batch, the far launch
-	// of the same block comes first).
+	// from the blocks up to q.  Staggered: for the channels s with (s / class_w) mod T == q mod T, every block;
+	// otherwise for all channels when q mod T == 0.  Both ways a channel's periods j are covered exactly once, and the
+	// near tier's window of a channel lies inside one far window of that channel (t_far is a multiple of t_batch, the
+	// far launch of the same block comes first).  Folded, the near tier starts at partition 3: period q+3+t gets every
+	// partition p >= 3+t (all of them involve blocks up to q only), the fused kernel sums the rest, 0 .. 2+t.
 	int launch_tiers0(FirLevel &L, long q, cudaStream_t bs, bool serial)
 	{
 		bool any = false;
 		for (int i = (t_far > 0) ? 1 : 0; i >= 0; --i) {
 			const int T = i ? t_far : t_batch;
-			// K residue classes of channels take turns, one launch every T / K blocks: K = T when staggered, 1 for whole
+			// K classes of channel groups take turns, one launch every T / K blocks: K = T when staggered, 1 for whole
 			// launches, far_classes for the far tier in between
 			const int K = stagger ? T : (i ? far_classes : 1);
+			const int w = class_w;
 			const int period = T / K;
 			if (q % period != 0) continue;
 			const int g = (int) ((q / period) % K);
-			if (n_sel <= g) continue;
+			if (n_sel <= g * w) continue;
+			int n_y = 0;   // channels of class g
+			for (int G = g; G * w < n_sel; G += K) n_y += (n_sel - G * w < w) ? n_sel - G * w : w;
 			if (!any && !serial) CUDA_TRY(cudaStreamWaitEvent(bs, ev_main, 0), return -1);
 			any = true;
 			MacBatchArgs b = {};
@@ -1994,13 +2032,14 @@ struct FirOp : Op {
 			b.V = i ? d_V2 : d_V; b.n_slots = 2 * T;
 			b.h_ch_stride = (fc == 1) ? 0 : (long) L.P * L.B;
 			b.pf = i ? 2 + far_e : 2;
-			b.p_lo = T + b.pf; b.p_hi = (i == 0 && t_far > 0) ? t_far + 2 + far_e : L.P;
+			b.p_lo = (i == 0 && fold) ? b.pf + 1 : T + b.pf;
+			b.p_hi = (i == 0 && t_far > 0) ? t_far + 2 + far_e : L.P;
 			if (i == 0 && t_far > 0) { b.Vin = d_V2; b.vin_slots = 2 * t_far; }
-			b.s_first = g; b.s_step = K;
+			b.g = g; b.K = K; b.w = w;
 			int threads = batch_threads_for(T);
 			if ((batch_threads == 128 || batch_threads == 64) && batch_threads < threads) threads = batch_threads;
 			if (L.B < threads) threads = L.B;
-			dim3 grid(L.B / threads, (n_sel - g + K - 1) / K);
+			dim3 grid(L.B / threads, n_y);
 			// whole launches of the far tier: at most one CTA per SM (DSP_B200_FIR_FAR_SMEM_KB, 0 = no cap)
 			static const long far_kb = getenv("DSP_B200_FIR_FAR_SMEM_KB") ? atol(getenv("DSP_B200_FIR_FAR_SMEM_KB")) : 0;
 			launch_mac_batch(T, fc == 1, grid, threads, bs, b, i ? "fir_mac_batch_far" : "fir_mac_batch",
@@ -2273,6 +2312,8 @@ struct FirOp : Op {
 							if (cudaEvent_t e = ev_bs_at[(L0.blk - 3) & 3]) CUDA_TRY(cudaStreamWaitEvent(ls, e, 0), return -1);
 							f.init = d_V + (size_t) (L0.blk % (2 * t_batch)) * n_sel * B0;
 						}
+						f.blk = L0.blk;
+						f.cls_T = t_batch; f.cls_K = stagger ? t_batch : 1; f.cls_w = class_w;
 					}
 					else if (tail_pf == 2 && L0.blk >= 2) {
 						// Y of this block was launched two blocks ago (advance_tail0)
