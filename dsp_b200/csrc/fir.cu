@@ -23,20 +23,22 @@
 //                       pf = P partitions of S_j from registers, + Y_j (below), inverse transform, overlap.
 //                       On single-level plans it reads the caller's interleaved block and writes the caller's
 //                       result itself (clusters of four adjacent channels share the rows through DSMEM); with a
-//                       batch tier it starts from V_j and sums the partitions the tier left out: 0 .. 2+t when V_j
-//                       came from the launch after block j-3-t ("folded": no k_fir_mac).
+//                       batch tier it starts from V_j and sums the partitions the tier left out: 0 .. la-1+t when
+//                       V_j came from the launch after block j-la-t ("folded": no k_fir_mac; the look-ahead la is 3,
+//                       or 2 on the full-wave plan below).
 //   k_fir_mac           Y_j = V_j + sum_{pf<=p<pf+T} X_{j-p} . H_p on a side stream, a block period ahead (the
 //                       blocks it needs were complete pf periods ago): the HBM-streaming kernel
 //   k_fir_mac_batch<T>  V_j = sum_{p>=pf+T} X_{j-p} . H_p for T periods at once (filter rows slide through a
 //                       register window: every FDL and filter row is read once per T outputs); folded, the near
-//                       tier also takes every partition p < pf+T whose block is complete (the triangle p >= 3+t)
+//                       tier also takes every partition p < pf+T whose block is complete (the triangle p >= la+t)
 //   k_fir_mac_bulk<8>   calls that bring several whole 8192-blocks: all partitions of up to 8 new blocks in
 //                       one pass, with one forward and one inverse launch (k_fir_fwd / k_fir_inv, gridDim.y)
 //   k_fir_stash/unstash interleaved <-> per-channel copies for multi-level plans and ragged calls
 // Spectra are stored "packed": B complex per row, bin 0 = (DC.re, Nyquist.re); rows are 16 B bytes
 // long, 128-byte aligned.  131072 taps, 4096-frame blocks: 1040 algorithmic bytes per sample for the plain
 // uniform scheme, 508 with the fused kernel + per-block MAC + time-batched tail, 476 with the per-block MAC folded
-// into the fused kernel, 440 with the near tier taking the triangle of partitions its rows already meet.
+// into the fused kernel, 440 with the near tier taking the triangle of partitions its rows already meet, 360 on the
+// full-wave plan (256 channels fill the GPU with fused CTAs: a near tier of depth 8 that looks two blocks ahead).
 //
 // Calls that are not whole aligned blocks take the general path, exact for ANY frames-per-call
 // pattern: with R_j = sum_{1<=p<P0} X_{j-p} . H_p (completed level-0 blocks only)
@@ -279,10 +281,11 @@ struct L0Args {
 	long h_ch_stride;
 	int P, slot;             // P: partitions summed (1, 2: compiled in; more: the folded tail, k_fir_level0<N, 0>)
 	// folded tail (cls_T > 0): block blk's V_j of channel s comes from the near-tier launch of its class
-	// c = (s / cls_w) % cls_K that covers j, made t = (blk - 3 - c) mod cls_T blocks earlier; it holds the partitions
-	// from 3 + t on, the kernel sums 0 .. 2 + t (all P while no launch has covered j)
+	// c = (s / cls_w) % cls_K that covers j, made la + t blocks earlier, t = (blk - la - c) mod cls_T (la: the look-ahead,
+	// 3 or 2); it holds the partitions from la + t on, the kernel sums 0 .. la - 1 + t (all P = cls_T + la - 1 while no
+	// launch has covered j)
 	long blk;
-	int cls_T, cls_K, cls_w;
+	int cls_T, cls_K, cls_w, la;
 	double *out;             // [s][out_ch_stride]: first half + carry
 	long out_ch_stride;
 	double *carry;           // [s][N]
@@ -400,8 +403,8 @@ __device__ __forceinline__ double2 cmac(double2 acc, double2 x, double2 h)
 #define FIR_L0_MAXNREG 128
 #endif
 // P: partitions summed, or 0: a run-time count of at most a.P (single-level plans with a batch tier: the "folded" tail,
-// partitions 0 .. 2+t of a channel whose V_j came from the near-tier launch after block j-3-t, so that no per-block MAC
-// and no Y spectrum round trip are needed)
+// partitions 0 .. la-1+t of a channel whose V_j came from the near-tier launch after block j-la-t, so that no per-block
+// MAC and no Y spectrum round trip are needed)
 template <int N, int P, bool CL = false>
 __global__ void __launch_bounds__(FftCfg<N>::THREADS) __maxnreg__((N == 4096) ? FIR_L0_MAXNREG : 128) k_fir_level0(L0Args a)
 {
@@ -631,8 +634,8 @@ __global__ void __launch_bounds__(FftCfg<N>::THREADS) __maxnreg__((N == 4096) ? 
 			// loop a different number of times: no barrier inside.)
 			int np = a.P;
 			if (a.cls_T > 0) {
-				const long d = a.blk - 3 - (s >> (__ffs(a.cls_w) - 1)) % a.cls_K;
-				if (d >= 0) np = 3 + (int) (d % a.cls_T);
+				const long d = a.blk - a.la - (s >> (__ffs(a.cls_w) - 1)) % a.cls_K;
+				if (d >= 0) np = a.la + (int) (d % a.cls_T);
 			}
 #pragma unroll 1
 			for (int p = 1; p < np; ++p) mac_partition(p);
@@ -1005,7 +1008,8 @@ __global__ void __launch_bounds__(256, FIR_MAC_MINB) k_fir_tail(TailArgs a)
 	}
 }
 
-constexpr int FIR_T_BATCH = 4;   // default depth of the near tier; DSP_B200_FIR_T=6|8 selects the other instantiations
+constexpr int FIR_T_BATCH = 4;   // default depth of the near tier; DSP_B200_FIR_T=4|6|8 selects an instantiation
+constexpr int FIR_T_FULL_WAVE = 8;   // ... on full-wave plans (FirOp::plan) of at least 2 * 8 + 3 partitions
 constexpr int FIR_T_FAR = 8;      // default depth of the far tier (DSP_B200_FIR_T2=0|8|12|16) ...
 constexpr int FIR_FAR_MIN_P = 48; // ... on levels of at least this many partitions
 
@@ -1461,10 +1465,20 @@ struct FirOp : Op {
 	cudaEvent_t ev_bs[8] = {};           // after the tier launches of a block (ring), ev_bs_last: the latest one
 	int ev_bs_n = 0;
 	cudaEvent_t ev_bs_last = nullptr;
-	// folded tail: the fused kernel of block j starts from V_j, which the tier launches up to block j-3 complete;
+	// folded tail: the fused kernel of block j starts from V_j, which the tier launches up to block j-la complete;
 	// ev_bs_at[q & 3] = ev_bs_last as it was after block q
 	bool fold = false;
 	cudaEvent_t ev_bs_at[4] = {};
+	// look-ahead of the folded near tier: its launch after block q covers the periods q+la .. q+la+T-1, from partition
+	// la + t on for period q+la+t (every block involved is complete).  3 by default; 2 on the full-wave plan (below),
+	// where the fused kernel is the step's critical path and one partition fewer per block shortens it.
+	// Invariants (T = t_batch):
+	//  - the V ring of 2 T slots is safe for T >= la: the next write to V_j's slot is for period j + 2T, by a launch after
+	//    block j + T - la + 1 > j or later, and launches only start once the fused kernel of their block is complete;
+	//  - FDL row j mod P (X_{j-P} until block j overwrites it) is read by the tier launches after blocks up to j-la-1;
+	//    the fused kernel of block j waits for the launches up to j-la, which covers them;
+	//  - the general path (wait_batch_for) still waits for every launch made so far.
+	int la = 3;
 	// staggered folded plans: the classes take turns over groups of class_w adjacent channels (1 otherwise), so that
 	// the four channels of a cluster sum the same number of partitions and finish together
 	int class_w = 1;
@@ -1494,8 +1508,8 @@ struct FirOp : Op {
 
 	// partitions level 0's fused kernel sums on whole aligned blocks: at most, and (folded: once every class has had a
 	// near-tier launch) at least
-	int l0_parts() const { return fold ? t_batch + 2 : (lv[0].P < 2) ? lv[0].P : 2; }
-	int l0_parts_min() const { return fold ? 3 : l0_parts(); }
+	int l0_parts() const { return fold ? t_batch + la - 1 : (lv[0].P < 2) ? lv[0].P : 2; }
+	int l0_parts_min() const { return fold ? la : l0_parts(); }
 
 	std::string describe() const override
 	{
@@ -1505,9 +1519,9 @@ struct FirOp : Op {
 		for (int l = 0; l < n_levels && n < (int) sizeof(buf) - 64; ++l)
 			n += snprintf(buf + n, sizeof(buf) - n, "%s{\"B\":%d,\"P\":%d}", l ? "," : "", lv[l].B, lv[l].P);
 		n += snprintf(buf + n, sizeof(buf) - n, "],\"t_batch\":%d,\"t_far\":%d,\"far_e\":%d,\"far_classes\":%d,\"stagger\":%d,\"class_width\":%d,\"merge\":%d,\"tail_pf\":%d,"
-		              "\"l0_parts\":%d,\"l0_parts_min\":%d,\"bulk\":%d,\"pipe\":%d,\"pipe_pf\":%d,",
-		              t_batch, t_far, far_e, far_classes, stagger ? 1 : 0, class_w, merge_tail ? 1 : 0, tail_pf, l0_parts(), l0_parts_min(), nb_max,
-		              use_pipe ? 1 : 0, pipe_pf);
+		              "\"l0_parts\":%d,\"l0_parts_min\":%d,\"lookahead\":%d,\"bulk\":%d,\"pipe\":%d,\"pipe_pf\":%d,",
+		              t_batch, t_far, far_e, far_classes, stagger ? 1 : 0, class_w, merge_tail ? 1 : 0, tail_pf, l0_parts(), l0_parts_min(), la,
+		              nb_max, use_pipe ? 1 : 0, pipe_pf);
 		snprintf(buf + n, sizeof(buf) - n, "\"replans\":%d,\"paths\":{\"fused\":%ld,\"cluster\":%ld,\"pipe\":%ld,\"bulk\":%ld,\"general\":%ld,\"head\":%ld}}",
 		         replans, n_fused, n_cluster, n_pipe, n_bulk, n_general, n_head);
 		return buf;
@@ -1539,6 +1553,7 @@ struct FirOp : Op {
 		ev_bs_last = nullptr; ev_bs_n = 0;
 		for (cudaEvent_t &e : ev_bs_at) e = nullptr;
 		fold = false;
+		la = 3;
 		class_w = 1;
 		for (cudaEvent_t &e : ev_tail) { if (e) cudaEventDestroy(e); e = nullptr; }
 		for (cudaEvent_t &e : ev_join) { if (e) cudaEventDestroy(e); e = nullptr; }
@@ -1652,8 +1667,15 @@ struct FirOp : Op {
 					CUDA_TRY(cudaEventCreateWithFlags(&ev_hot_in, cudaEventDisableTiming), return -1);
 					CUDA_TRY(cudaEventCreateWithFlags(&ev_hot_out, cudaEventDisableTiming), return -1);
 				}
+				// The fold pays once the fused kernel's CTAs outnumber half the SMs (see `fold` below).  Those plans are
+				// "full-wave": the fused kernel fills the GPU and carries most of the bytes, so the near tier goes deeper
+				// (T = 8 reads every FDL and filter row once per 8 periods instead of 4: 440 -> 388 B/sample on the
+				// headline) and, with one tier, looks two blocks ahead instead of three (la = 2: 360 B/sample).
+				const int cpb = (L.B / 16 >= 256) ? 1 : 256 / (L.B / 16);   // FftCfg<B>::CPB
+				const bool fold_pays = 2 * ceil_div(n_sel, cpb) > sm_count();
+				const bool full_wave = l == 0 && !use_pipe && direct_io && fold_pays;
 				const char *nb = getenv("DSP_B200_FIR_NO_BATCH");
-				int tb = FIR_T_BATCH;
+				int tb = (full_wave && L.P >= 2 * FIR_T_FULL_WAVE + pf + 1) ? FIR_T_FULL_WAVE : FIR_T_BATCH;
 				if (const char *e = getenv("DSP_B200_FIR_T")) tb = (atoi(e) == 8) ? 8 : (atoi(e) == 6) ? 6 : 4;
 				if (use_pipe) tb = PIPE_TB;   // the pipeline kernel's batch depth is compiled in (one channel residue per block)
 				if (L.P >= 2 * tb + pf + 1 && !(nb && nb[0] == '1')) {
@@ -1671,7 +1693,9 @@ struct FirOp : Op {
 						// far tier: partitions >= t_far + 2, T = t_far periods per launch; only when the level is long
 						// enough for it to pay (the near tier keeps partitions t_batch + 2 .. t_far + 1)
 						// (at 32 partitions the second tier saves bytes but no time; at 64 partitions -- 2048-frame blocks --
-						// it pays)
+						// it pays behind a near tier of 4.  On the full-wave plan the near tier of 8 leaves no far tier of
+						// 8: one staggered tier of 8 looking two blocks ahead measured 9% faster than tiers 4 + 8 at 256
+						// channels of 2048 frames, and 5% faster than tiers 8 + 16, DESIGN.md K2)
 						int t2 = (L.P >= FIR_FAR_MIN_P) ? FIR_T_FAR : 0;
 						if (const char *e = getenv("DSP_B200_FIR_T2")) t2 = atoi(e);
 						if (!batch_depth_ok(t2) || t2 <= t_batch || t2 % t_batch != 0 || L.P < 2 * t2 + pf + t_batch) t2 = 0;
@@ -1706,16 +1730,15 @@ struct FirOp : Op {
 					if (getenv("DSP_B200_FIR_PIPE_STATS")) d_stats = dev_alloc<long long>(8 * 1024);
 				}
 				// Folded tail (single level, direct I/O, a batch tier): the fused kernel starts from the near tier's V_j and
-				// sums what that tier leaves out, 3 .. t_batch+2 partitions (launch_tiers0) -- no per-block MAC, no Y spectrum
-				// through HBM (440 instead of 508 bytes per sample on the headline, DESIGN.md K2).  Only when the fused
-				// kernel's CTAs outnumber half the SMs: with fewer, the per-block MAC streams on the SMs the fused kernel
-				// leaves idle, and moving its partitions into the few fused CTAs lengthens the step (64 channels of 4096
-				// frames: 8% slower folded, 256: 6% faster).
+				// sums what that tier leaves out, la .. t_batch+la-1 partitions (launch_tiers0) -- no per-block MAC, no Y
+				// spectrum through HBM (DESIGN.md K2).  Only when the fused kernel's CTAs outnumber half the SMs: with
+				// fewer, the per-block MAC streams on the SMs the fused kernel leaves idle, and moving its partitions into
+				// the few fused CTAs lengthens the step (64 channels of 4096 frames: 8% slower folded, 256: 6% faster).
 				// DSP_B200_FIR_FOLD=1 / 0 force either form (tests, measurements); the merged grid is a per-block MAC.
+				// The look-ahead of 2 is for full-wave plans with one tier only (a far tier keeps 3).
 				const char *fe = getenv("DSP_B200_FIR_FOLD");
-				const int cpb = (L.B / 16 >= 256) ? 1 : 256 / (L.B / 16);   // FftCfg<B>::CPB
-				const bool fold_pays = 2 * ceil_div(n_sel, cpb) > sm_count();
 				fold = l == 0 && !use_pipe && direct_io && t_batch > 0 && !merge_tail && (fe ? fe[0] == '1' : fold_pays);
+				la = (fold && full_wave && t_far == 0) ? 2 : 3;
 				// staggered classes of up to 4 adjacent channels (a cluster's four when there are enough channels for every
 				// class to have a whole group): all CTAs of a cluster sum the same partitions, and a cluster that finishes
 				// early hands its SMs to the queued batch CTAs at once instead of waiting for its slowest channel
@@ -2004,12 +2027,13 @@ struct FirOp : Op {
 	}
 
 	// Tier launches after block q of a single-level plan (far tier first: the near tier starts from its sums).  A tier
-	// of depth T produces V_j = (farther tier's V_j) + sum_{p in tier} X_{j-p} H_p for the T periods j = q+3 .. q+2+T
-	// from the blocks up to q.  Staggered: for the channels s with (s / class_w) mod T == q mod T, every block;
-	// otherwise for all channels when q mod T == 0.  Both ways a channel's periods j are covered exactly once, and the
-	// near tier's window of a channel lies inside one far window of that channel (t_far is a multiple of t_batch, the
-	// far launch of the same block comes first).  Folded, the near tier starts at partition 3: period q+3+t gets every
-	// partition p >= 3+t (all of them involve blocks up to q only), the fused kernel sums the rest, 0 .. 2+t.
+	// of depth T produces V_j = (farther tier's V_j) + sum_{p in tier} X_{j-p} H_p for the T periods j = q+la ..
+	// q+la-1+T from the blocks up to q (la = 3 unless folded on a full-wave plan; the far tier works far_e periods further
+	// ahead).  Staggered: for the channels s with (s / class_w) mod T == q mod T, every block; otherwise for all channels
+	// when q mod T == 0.  Both ways a channel's periods j are covered exactly once, and the near tier's window of a
+	// channel lies inside one far window of that channel (t_far is a multiple of t_batch, the far launch of the same
+	// block comes first).  Folded, the near tier starts at partition la: period q+la+t gets every partition p >= la+t
+	// (all of them involve blocks up to q only), the fused kernel sums the rest, 0 .. la-1+t.
 	int launch_tiers0(FirLevel &L, long q, cudaStream_t bs, bool serial)
 	{
 		bool any = false;
@@ -2031,8 +2055,8 @@ struct FirOp : Op {
 			b.fdl = L.fdl; b.H = L.H; b.N = L.B; b.P = L.P; b.n_sel = n_sel; b.q = q;
 			b.V = i ? d_V2 : d_V; b.n_slots = 2 * T;
 			b.h_ch_stride = (fc == 1) ? 0 : (long) L.P * L.B;
-			b.pf = i ? 2 + far_e : 2;
-			b.p_lo = (i == 0 && fold) ? b.pf + 1 : T + b.pf;
+			b.pf = i ? 2 + far_e : la - 1;
+			b.p_lo = (i == 0 && fold) ? la : T + b.pf;
 			b.p_hi = (i == 0 && t_far > 0) ? t_far + 2 + far_e : L.P;
 			if (i == 0 && t_far > 0) { b.Vin = d_V2; b.vin_slots = 2 * t_far; }
 			b.g = g; b.K = K; b.w = w;
@@ -2054,8 +2078,8 @@ struct FirOp : Op {
 	}
 
 	// The main stream may only go on with block `blk` of a single-level tail plan once the tier launches that read FDL
-	// row blk % P (those after the blocks up to blk-4) are complete.  The fused kernel's path gets that from waiting
-	// for Y_blk (whose MAC waited for the launches up to blk-3) or, folded, for the launches up to blk-3 themselves;
+	// row blk % P (those after the blocks up to blk-la-1) are complete.  The fused kernel's path gets that from waiting
+	// for Y_blk (whose MAC waited for the launches up to blk-3) or, folded, for the launches up to blk-la themselves;
 	// the general path waits here, for all of them.
 	int wait_batch_for(long blk, cudaStream_t st)
 	{
@@ -2305,15 +2329,16 @@ struct FirOp : Op {
 						ls = hot;
 					}
 					if (fold) {
-						// V_j: complete once the tier launches up to block j-3 are, and nothing overwrites its slot before
-						// block j+2's launch; those launches have read FDL row j % P (blocks up to j-4 read it) as well.
-						// Before block 3 no launch has covered V_j: it is zero (the blocks it sums do not exist).
-						if (L0.blk >= 3) {
-							if (cudaEvent_t e = ev_bs_at[(L0.blk - 3) & 3]) CUDA_TRY(cudaStreamWaitEvent(ls, e, 0), return -1);
+						// V_j: complete once the tier launches up to block j-la are, and nothing overwrites its slot before
+						// this kernel is done (see `la`); those launches have read FDL row j % P (blocks up to j-la-1 read
+						// it) as well.  Before block la no launch has covered V_j: it is zero (the blocks it sums do not
+						// exist).
+						if (L0.blk >= la) {
+							if (cudaEvent_t e = ev_bs_at[(L0.blk - la) & 3]) CUDA_TRY(cudaStreamWaitEvent(ls, e, 0), return -1);
 							f.init = d_V + (size_t) (L0.blk % (2 * t_batch)) * n_sel * B0;
 						}
 						f.blk = L0.blk;
-						f.cls_T = t_batch; f.cls_K = stagger ? t_batch : 1; f.cls_w = class_w;
+						f.cls_T = t_batch; f.cls_K = stagger ? t_batch : 1; f.cls_w = class_w; f.la = la;
 					}
 					else if (tail_pf == 2 && L0.blk >= 2) {
 						// Y of this block was launched two blocks ago (advance_tail0)

@@ -3,11 +3,12 @@
 measured step time.  bench.py's fir_bytes_model charges every single-level tail plan with a per-block k_fir_mac; on
 plans with a folded tail (the default; describe() "l0_parts" > 2) there is none: the fused kernel reads lp filter rows and
 lp - 1 FDL rows, and V_j in place of Y_j.  A channel sums lp = l0_parts_min .. l0_parts partitions in turn (the near
-tier takes the rest of partitions 3 .. t_batch+1 of the periods it covers), lp is their mean; the near tier reads
-l0_parts - l0_parts_min filter rows more than bench.py says, the far tier costs what bench.py says.
+tier takes the rest of partitions la .. t_batch+la-2 of the periods it covers, la = the look-ahead), lp is their mean,
+la + (t_batch - 1) / 2; the near tier reads P - la FDL rows and P - la filter rows per launch, the far tier costs what
+bench.py says.
 
     python scripts/fir_bytes.py bench_line.json        # a bench.py result line: its plan, its step time
-    python scripts/fir_bytes.py --block 4096 --taps 131072 [--t 4] [--shared-ir] [--unfolded] [--step-us 186]
+    python scripts/fir_bytes.py --block 4096 --taps 131072 [--t 4] [--lookahead 3] [--shared-ir] [--unfolded] [--step-us 186]
 """
 import argparse
 import json
@@ -29,20 +30,25 @@ def folded_bytes_model(plan, h):
         lp = (lp_min + lp_max) / 2.0
         parts.pop("fir_mac")
         parts["fir_level0"] = 8 + 16 + 16.0 * (lp - 1) + 16.0 * lp * h + 16 + 8 + 8 + 8
-        # the near tier's filter rows H_3 .. H_{t_batch+1}, once per launch of t_batch periods
-        parts["fir_mac_batch"] += 16.0 * (lp_max - lp_min) * h / int(plan["t_batch"])
+        # bench.py charges the near tier the FDL rows from partition 3 and the filter rows from t_batch + 2.  Its launch
+        # streams the FDL rows from partition la (the look-ahead, describe() "lookahead") and the filter rows from
+        # lp_min on: X_la .. X_2 and H_{lp_min} .. H_{t_batch+1} more, once per launch of t_batch periods
+        T, la = int(plan["t_batch"]), int(plan.get("lookahead", 3))
+        parts["fir_mac_batch"] += 16.0 * ((3 - la) + (T + 2 - lp_min) * h) / T
         total = sum(parts.values())
     return total, parts
 
 
 def plan_from_args(a):
-    """The single-level plan FirOp::plan() makes for 2048..8192-frame blocks with the default knobs (no far tier below
-    48 partitions, the stagger from 16 tail partitions on)."""
+    """The single-level plan FirOp::plan() makes for 2048..8192-frame blocks at batch depth a.t and look-ahead a.lookahead
+    (3 when absent; the full-wave plan uses 2 with one tier) with the default knobs (no far tier below 48 partitions,
+    the stagger from 16 tail partitions on)."""
     P = -(-a.taps // a.block)
     t_far = 8 if P >= 48 and 8 > a.t and 8 % a.t == 0 and P >= 2 * 8 + 2 + a.t else 0
+    la = 3 if a.unfolded or t_far else int(getattr(a, "lookahead", None) or 3)
     return {"levels": [{"B": a.block, "P": P}], "tail_pf": 2, "t_batch": a.t, "t_far": t_far, "far_e": a.t if t_far else 0,
             "stagger": 1 if not t_far and P - a.t - 2 >= 16 else 0, "merge": 0, "pipe": 0, "pipe_pf": 0,
-            "l0_parts": 2 if a.unfolded else a.t + 2, "l0_parts_min": 2 if a.unfolded else 3}
+            "l0_parts": 2 if a.unfolded else a.t + la - 1, "l0_parts_min": 2 if a.unfolded else la, "lookahead": la}
 
 
 def main():
@@ -52,6 +58,7 @@ def main():
     ap.add_argument("--taps", type=int, default=131072)
     ap.add_argument("--channels", type=int, default=256)
     ap.add_argument("--t", type=int, default=4, help="batch depth (DSP_B200_FIR_T)")
+    ap.add_argument("--lookahead", type=int, default=3, choices=[2, 3], help="look-ahead of the folded near tier")
     ap.add_argument("--shared-ir", action="store_true")
     ap.add_argument("--unfolded", action="store_true", help="the per-block MAC form (DSP_B200_FIR_FOLD=0)")
     ap.add_argument("--step-us", type=float, help="measured step time")
@@ -68,7 +75,7 @@ def main():
         plan = plan_from_args(a)
     B = plan["levels"][-1]["B"]
     total, parts = folded_bytes_model(plan, h)
-    out = {"plan": {k: plan[k] for k in ("levels", "t_batch", "t_far", "stagger", "l0_parts", "l0_parts_min") if k in plan},
+    out = {"plan": {k: plan[k] for k in ("levels", "t_batch", "t_far", "stagger", "l0_parts", "l0_parts_min", "lookahead") if k in plan},
            "bytes_per_sample": total, "bytes_per_sample_by_kernel": parts, "bytes_per_step": total * C * B}
     if step_us:
         gbs = total * C * B / (step_us * 1e-6) / 1e9
