@@ -11,6 +11,7 @@
 #include "ops.h"
 #include "fft.cuh"
 #include "../../include/dsp_b200.h"
+#include <cassert>
 #include <cmath>
 #include <map>
 #include <mutex>
@@ -340,8 +341,12 @@ struct Shard {
 				else { dst = buf[1 + flip]; flip ^= 1; }
 			}
 			else {
-				if (last && cur != out) dst = out;
-				else if (last) { set_error("chain: in-place call on a rate-changing chain"); return -1; }
+				if (last) {
+					// never in place: dspb200_chain_run_device rejects in == out on such a chain before anything runs,
+					// and the host calls write their result to buf[3], which no operator reads
+					assert(cur != out);
+					dst = out;
+				}
 				else {
 					dst = buf[1 + flip];
 					flip ^= 1;
@@ -785,6 +790,12 @@ long dspb200_chain_run_device(dspb200_chain *c, int shard, long frames, const do
 	if (!c || shard < 0 || shard >= (int) c->shards.size() || !d_in || !d_out) return -1;
 	if (frames < 1) return 0;
 	Shard *s = c->shards[shard].get();
+	if (d_in == d_out && !s->ops.empty() && !s->ops.back()->inplace_ok) {
+		// checked before anything is enqueued: the operators ahead of the last one would otherwise already have
+		// filtered the caller's buffer in place and moved their state on
+		set_error("chain: in-place call on a chain whose last operator changes the frame count");
+		return -1;
+	}
 	CUDA_TRY(cudaSetDevice(s->device), return -1);
 	if (s->ensure_cap(frames)) return -1;
 	cudaStream_t st = (cudaStream_t) stream;   // NULL = the legacy default stream, as everywhere in CUDA

@@ -127,7 +127,9 @@ int  dspb200_chain_wait(dspb200_chain *c, unsigned long long ticket);
 
 /* Mode D: one shard, device-resident interleaved buffers of that shard's channel count,
  * enqueued on `stream` (a cudaStream_t; NULL = the legacy default stream), asynchronous.
- * d_in == d_out allowed only when no operator changes the frame count.  Returns output frames. */
+ * d_in == d_out is allowed unless the chain's last operator changes the frame count (resample, align); such a call
+ * is rejected before anything runs: it returns < 0 and leaves the buffer and the chain's state as they were.
+ * Returns output frames. */
 long dspb200_chain_run_device(dspb200_chain *c, int shard, long frames, const double *d_in,
                               double *d_out, void *stream);
 
