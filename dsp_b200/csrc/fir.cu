@@ -30,7 +30,9 @@
 //                       blocks it needs were complete pf periods ago): the HBM-streaming kernel
 //   k_fir_mac_batch<T>  V_j = sum_{p>=pf+T} X_{j-p} . H_p for T periods at once (filter rows slide through a
 //                       register window: every FDL and filter row is read once per T outputs); folded, the near
-//                       tier also takes every partition p < pf+T whose block is complete (the triangle p >= la+t)
+//                       tier also takes every partition p < pf+T whose block is complete (the triangle p >= la+t);
+//                       on the full-wave plan the same grid runs the mid-window pass of the class launched m blocks
+//                       earlier, which adds partitions la+t-m .. la-1+t to its periods t >= m (FirOp::pass_m)
 //   k_fir_mac_bulk<8>   calls that bring several whole 8192-blocks: all partitions of up to 8 new blocks in
 //                       one pass, with one forward and one inverse launch (k_fir_fwd / k_fir_inv, gridDim.y)
 //   k_fir_stash/unstash interleaved <-> per-channel copies for multi-level plans and ragged calls
@@ -38,7 +40,8 @@
 // long, 128-byte aligned.  131072 taps, 4096-frame blocks: 1040 algorithmic bytes per sample for the plain
 // uniform scheme, 508 with the fused kernel + per-block MAC + time-batched tail, 476 with the per-block MAC folded
 // into the fused kernel, 440 with the near tier taking the triangle of partitions its rows already meet, 360 on the
-// full-wave plan (256 channels fill the GPU with fused CTAs: a near tier of depth 8 that looks two blocks ahead).
+// full-wave plan (256 channels fill the GPU with fused CTAs: a near tier of depth 8 that looks two blocks ahead), 334
+// with the mid-window pass (the fused kernel sums 2 .. 5 partitions instead of 2 .. 9).
 //
 // Calls that are not whole aligned blocks take the general path, exact for ANY frames-per-call
 // pattern: with R_j = sum_{1<=p<P0} X_{j-p} . H_p (completed level-0 blocks only)
@@ -283,9 +286,10 @@ struct L0Args {
 	// folded tail (cls_T > 0): block blk's V_j of channel s comes from the near-tier launch of its class
 	// c = (s / cls_w) % cls_K that covers j, made la + t blocks earlier, t = (blk - la - c) mod cls_T (la: the look-ahead,
 	// 3 or 2); it holds the partitions from la + t on, the kernel sums 0 .. la - 1 + t (all P = cls_T + la - 1 while no
-	// launch has covered j)
+	// launch has covered j).  pass_m > 0: the class's mid-window pass after block j-la-t+pass_m has added partitions
+	// la+t-pass_m .. la-1+t for t >= pass_m, the kernel sums 0 .. la-1+t-pass_m there
 	long blk;
-	int cls_T, cls_K, cls_w, la;
+	int cls_T, cls_K, cls_w, la, pass_m;
 	double *out;             // [s][out_ch_stride]: first half + carry
 	long out_ch_stride;
 	double *carry;           // [s][N]
@@ -630,12 +634,17 @@ __global__ void __launch_bounds__(FftCfg<N>::THREADS) __maxnreg__((N == 4096) ? 
 			for (int p = 1; p < P; ++p) mac_partition(p);
 		}
 		else {
-			// (d < 0: the class's first launch covers a later period.  The two transform groups of a 2048-point CTA may
-			// loop a different number of times: no barrier inside.)
+			// (d < 0: the class's first launch covers a later period.  d >= 0 and t >= pass_m: the pass after block
+			// j-la-t+pass_m <= j-la has run too.  The two transform groups of a 2048-point CTA may loop a different
+			// number of times: no barrier inside.)
 			int np = a.P;
 			if (a.cls_T > 0) {
 				const long d = a.blk - a.la - (s >> (__ffs(a.cls_w) - 1)) % a.cls_K;
-				if (d >= 0) np = a.la + (int) (d % a.cls_T);
+				if (d >= 0) {
+					int t = (int) (d % a.cls_T);
+					if (t >= a.pass_m) t -= a.pass_m;
+					np = a.la + t;
+				}
 			}
 #pragma unroll 1
 			for (int p = 1; p < np; ++p) mac_partition(p);
@@ -875,6 +884,11 @@ struct MacBatchArgs {
 	int p_lo, p_hi;       // partitions of this tier
 	const double2 *Vin;   // [slot][s][N], slot = j mod vin_slots: a farther tier's sums to start from (NULL: zero)
 	int vin_slots;
+	// the mid-window pass of the folded near tier in the same grid (pass_m > 0): rows y >= n_tier_y are the channels of
+	// class pass_g, whose tier launch after block q - pass_m covered the periods q+pf+1-pass_m .. q+pf+T-pass_m.  Its
+	// periods j = q+pf+1+t, t < T - pass_m, get the partitions p_lo+t .. p_lo+t+pass_m-1 added to V_j in place: pass_m
+	// FDL rows X_q .. X_{q-pass_m+1} and the filter rows p_lo .. p_lo+T-2
+	int n_tier_y, pass_g, pass_m;
 };
 
 #ifndef FIR_BATCH_PREFETCH
@@ -892,23 +906,30 @@ struct MacBatchCfg {
 #endif
 };
 
-template <int T, bool SHARED_H, bool DCW>
+// PASS: the mid-window pass role (MacBatchArgs::pass_m): the same sliding window with X rows m < x_hi, filter rows
+// p < h_hi and T - pass_m periods, V read and written in place by the thread that owns the element
+template <int T, bool SHARED_H, bool DCW, bool PASS = false>
 __device__ __forceinline__ void fir_mac_batch_body(const MacBatchArgs &a, int y)
 {
 	const int k = blockIdx.x * blockDim.x + threadIdx.x;
 	const int wl = __ffs(a.w) - 1;   // w: a power of two
-	const int s = ((a.g + a.K * (y >> wl)) << wl) + (y & (a.w - 1));
+	const int s = (((PASS ? a.pass_g : a.g) + a.K * (y >> wl)) << wl) + (y & (a.w - 1));
+	const int x_hi = PASS ? a.p_lo + a.pass_m : a.p_hi;
+	const int h_hi = PASS ? a.p_lo + T - 1 : a.p_hi;
+	const int n_t = PASS ? T - a.pass_m : T;
+	const double2 *Vin = PASS ? a.V : a.Vin;
+	const int vin_slots = PASS ? a.n_slots : a.vin_slots;
 	const double2 *fdl = a.fdl + (long) s * a.P * a.N + k;
 	const double2 *H = a.H + (long) s * a.h_ch_stride + k;
 	const bool dc = DCW && (k == 0);
 	const double2 zero = make_double2(0.0, 0.0);
 	double2 acc[T], hw[T];
-#define HROW(p) (((p) >= a.p_lo && (p) < a.p_hi) ? (SHARED_H ? __ldg(&H[(long) (p) * a.N]) : __ldcs(&H[(long) (p) * a.N])) : zero)
+#define HROW(p) (((p) >= a.p_lo && (p) < h_hi) ? (SHARED_H ? __ldg(&H[(long) (p) * a.N]) : __ldcs(&H[(long) (p) * a.N])) : zero)
 	int m = a.pf + 1;   // first row: the newest complete block, X_q
 #pragma unroll
 	for (int t = 0; t < T; ++t) {
 		const long j = a.q + a.pf + 1 + t;
-		acc[t] = a.Vin ? __ldcs(&a.Vin[((j % a.vin_slots) * a.n_sel + s) * (long) a.N + k]) : zero;
+		acc[t] = (Vin && t < n_t) ? __ldcs(&Vin[((j % vin_slots) * a.n_sel + s) * (long) a.N + k]) : zero;
 		hw[t] = HROW(m + t);
 	}
 	int slot = (int) (a.q % a.P);   // row of X_{q+pf+1-m} = X_q
@@ -930,10 +951,10 @@ __device__ __forceinline__ void fir_mac_batch_body(const MacBatchArgs &a, int y)
 	} while (0)
 #if FIR_BATCH_PREFETCH
 	// the eight loads of the NEXT four rows are issued before the current four are used; rows past the tier are zeros
-#define XROWG(mm, d) (((mm) + (d) < a.p_hi) ? XROW(d) : zero)
+#define XROWG(mm, d) (((mm) + (d) < x_hi) ? XROW(d) : zero)
 	double2 x0 = XROWG(m, 0), x1 = XROWG(m, 1), x2 = XROWG(m, 2), x3 = XROWG(m, 3);
 	double2 h0 = HROW(m + T), h1 = HROW(m + T + 1), h2 = HROW(m + T + 2), h3 = HROW(m + T + 3);
-	for (; m < a.p_hi; m += 4) {
+	for (; m < x_hi; m += 4) {
 		slot -= 4;
 		if (slot < 0) slot += a.P;
 		const int mn = m + 4;
@@ -948,7 +969,7 @@ __device__ __forceinline__ void fir_mac_batch_body(const MacBatchArgs &a, int y)
 	}
 #undef XROWG
 #else
-	for (; m + 4 <= a.p_hi; m += 4) {
+	for (; m + 4 <= x_hi; m += 4) {
 		// eight independent 16-byte loads in flight per thread, as in k_fir_mac
 		const double2 x0 = XROW(0), x1 = XROW(1), x2 = XROW(2), x3 = XROW(3);
 		const double2 h0 = HROW(m + T), h1 = HROW(m + T + 1), h2 = HROW(m + T + 2), h3 = HROW(m + T + 3);
@@ -959,7 +980,7 @@ __device__ __forceinline__ void fir_mac_batch_body(const MacBatchArgs &a, int y)
 		slot -= 4;
 		if (slot < 0) slot += a.P;
 	}
-	for (; m < a.p_hi; ++m) {
+	for (; m < x_hi; ++m) {
 		const double2 x0 = XROW(0);
 		const double2 h0 = HROW(m + T);
 		STEP(x0, h0);
@@ -972,14 +993,19 @@ __device__ __forceinline__ void fir_mac_batch_body(const MacBatchArgs &a, int y)
 #pragma unroll
 	for (int t = 0; t < T; ++t) {
 		const long j = a.q + a.pf + 1 + t;
-		a.V[((j % a.n_slots) * a.n_sel + s) * (long) a.N + k] = acc[t];
+		if (t < n_t) a.V[((j % a.n_slots) * a.n_sel + s) * (long) a.N + k] = acc[t];
 	}
 }
 
 template <int T, bool SHARED_H>
 __global__ void __launch_bounds__(MacBatchCfg<T>::THREADS, MacBatchCfg<T>::MINB) k_fir_mac_batch(MacBatchArgs a)
 {
-	if (blockIdx.x == 0 && threadIdx.x < 32) fir_mac_batch_body<T, SHARED_H, true>(a, blockIdx.y);   // the warp that holds the packed bin 0
+	const bool dcw = blockIdx.x == 0 && threadIdx.x < 32;   // the warp that holds the packed bin 0
+	if (a.pass_m > 0 && (int) blockIdx.y >= a.n_tier_y) {
+		if (dcw) fir_mac_batch_body<T, SHARED_H, true, true>(a, (int) blockIdx.y - a.n_tier_y);
+		else fir_mac_batch_body<T, SHARED_H, false, true>(a, (int) blockIdx.y - a.n_tier_y);
+	}
+	else if (dcw) fir_mac_batch_body<T, SHARED_H, true>(a, blockIdx.y);
 	else fir_mac_batch_body<T, SHARED_H, false>(a, blockIdx.y);
 }
 
@@ -1008,7 +1034,7 @@ __global__ void __launch_bounds__(256, FIR_MAC_MINB) k_fir_tail(TailArgs a)
 	}
 }
 
-constexpr int FIR_T_BATCH = 4;   // default depth of the near tier; DSP_B200_FIR_T=4|6|8 selects an instantiation
+constexpr int FIR_T_BATCH = 4;   // default depth of the near tier; DSP_B200_FIR_T=4|6|8|12 selects an instantiation
 constexpr int FIR_T_FULL_WAVE = 8;   // ... on full-wave plans (FirOp::plan) of at least 2 * 8 + 3 partitions
 constexpr int FIR_T_FAR = 8;      // default depth of the far tier (DSP_B200_FIR_T2=0|8|12|16) ...
 constexpr int FIR_FAR_MIN_P = 48; // ... on levels of at least this many partitions
@@ -1479,6 +1505,19 @@ struct FirOp : Op {
 	//    the fused kernel of block j waits for the launches up to j-la, which covers them;
 	//  - the general path (wait_batch_for) still waits for every launch made so far.
 	int la = 3;
+	// mid-window pass (staggered full-wave plans with one tier, la = 2; DSP_B200_FIR_PASS=0|m, default T/2): the grid
+	// launched after block q' also runs a pass for the class whose tier launch came after block q = q' - pass_m.  For
+	// its periods q+la+t with t >= pass_m it adds partitions la+t-pass_m .. la-1+t to V in place (blocks q'-pass_m+1 ..
+	// q'), and the fused kernel sums 0 .. la-1+t-pass_m there: la .. la-1+max(pass_m, T-pass_m) partitions instead of
+	// la .. la-1+T.  Invariants, in addition to those of `la`:
+	//  - the pass after q' reads X_{q'} and waits for the fused kernel of block q', like the tier launch after q';
+	//  - the fused kernel of block j = q+la+t, t >= pass_m, waits for the launches up to j-la = q+t >= q', the pass included;
+	//  - V slots: the pass touches the periods q+la+pass_m .. q+la+T-1; the class's next tier launch (after q+T) writes
+	//    q+T+la .. q+2T+la-1: disjoint in the ring of 2T slots; their next writer, the tier launch after q+2T, comes after
+	//    the fused kernels that read them;
+	//  - FDL: the pass reads only rows newer than the tier launch of the same grid does (q'-pass_m+1 .. q'); the first
+	//    block to overwrite one, q'-pass_m+1+P, waits for the launches up to q'-pass_m+1+P-la >= q' (P >= 2T+3).
+	int pass_m = 0;
 	// staggered folded plans: the classes take turns over groups of class_w adjacent channels (1 otherwise), so that
 	// the four channels of a cluster sum the same number of partitions and finish together
 	int class_w = 1;
@@ -1510,6 +1549,8 @@ struct FirOp : Op {
 	// near-tier launch) at least
 	int l0_parts() const { return fold ? t_batch + la - 1 : (lv[0].P < 2) ? lv[0].P : 2; }
 	int l0_parts_min() const { return fold ? la : l0_parts(); }
+	// at most, once every class has had its mid-window pass (l0_parts() without one)
+	int l0_parts_steady() const { return fold ? la - 1 + ((pass_m > t_batch - pass_m) ? pass_m : t_batch - pass_m) : l0_parts(); }
 
 	std::string describe() const override
 	{
@@ -1519,9 +1560,9 @@ struct FirOp : Op {
 		for (int l = 0; l < n_levels && n < (int) sizeof(buf) - 64; ++l)
 			n += snprintf(buf + n, sizeof(buf) - n, "%s{\"B\":%d,\"P\":%d}", l ? "," : "", lv[l].B, lv[l].P);
 		n += snprintf(buf + n, sizeof(buf) - n, "],\"t_batch\":%d,\"t_far\":%d,\"far_e\":%d,\"far_classes\":%d,\"stagger\":%d,\"class_width\":%d,\"merge\":%d,\"tail_pf\":%d,"
-		              "\"l0_parts\":%d,\"l0_parts_min\":%d,\"lookahead\":%d,\"bulk\":%d,\"pipe\":%d,\"pipe_pf\":%d,",
-		              t_batch, t_far, far_e, far_classes, stagger ? 1 : 0, class_w, merge_tail ? 1 : 0, tail_pf, l0_parts(), l0_parts_min(), la,
-		              nb_max, use_pipe ? 1 : 0, pipe_pf);
+		              "\"l0_parts\":%d,\"l0_parts_min\":%d,\"l0_parts_steady\":%d,\"lookahead\":%d,\"pass_m\":%d,\"bulk\":%d,\"pipe\":%d,\"pipe_pf\":%d,",
+		              t_batch, t_far, far_e, far_classes, stagger ? 1 : 0, class_w, merge_tail ? 1 : 0, tail_pf, l0_parts(), l0_parts_min(),
+		              l0_parts_steady(), la, pass_m, nb_max, use_pipe ? 1 : 0, pipe_pf);
 		snprintf(buf + n, sizeof(buf) - n, "\"replans\":%d,\"paths\":{\"fused\":%ld,\"cluster\":%ld,\"pipe\":%ld,\"bulk\":%ld,\"general\":%ld,\"head\":%ld}}",
 		         replans, n_fused, n_cluster, n_pipe, n_bulk, n_general, n_head);
 		return buf;
@@ -1554,6 +1595,7 @@ struct FirOp : Op {
 		for (cudaEvent_t &e : ev_bs_at) e = nullptr;
 		fold = false;
 		la = 3;
+		pass_m = 0;
 		class_w = 1;
 		for (cudaEvent_t &e : ev_tail) { if (e) cudaEventDestroy(e); e = nullptr; }
 		for (cudaEvent_t &e : ev_join) { if (e) cudaEventDestroy(e); e = nullptr; }
@@ -1676,7 +1718,7 @@ struct FirOp : Op {
 				const bool full_wave = l == 0 && !use_pipe && direct_io && fold_pays;
 				const char *nb = getenv("DSP_B200_FIR_NO_BATCH");
 				int tb = (full_wave && L.P >= 2 * FIR_T_FULL_WAVE + pf + 1) ? FIR_T_FULL_WAVE : FIR_T_BATCH;
-				if (const char *e = getenv("DSP_B200_FIR_T")) tb = (atoi(e) == 8) ? 8 : (atoi(e) == 6) ? 6 : 4;
+				if (const char *e = getenv("DSP_B200_FIR_T")) tb = (atoi(e) == 12) ? 12 : (atoi(e) == 8) ? 8 : (atoi(e) == 6) ? 6 : 4;
 				if (use_pipe) tb = PIPE_TB;   // the pipeline kernel's batch depth is compiled in (one channel residue per block)
 				if (L.P >= 2 * tb + pf + 1 && !(nb && nb[0] == '1')) {
 					t_batch = tb;
@@ -1739,6 +1781,12 @@ struct FirOp : Op {
 				const char *fe = getenv("DSP_B200_FIR_FOLD");
 				fold = l == 0 && !use_pipe && direct_io && t_batch > 0 && !merge_tail && (fe ? fe[0] == '1' : fold_pays);
 				la = (fold && full_wave && t_far == 0) ? 2 : 3;
+				// the mid-window pass halves the fused kernel's triangle (see `pass_m`): 360 -> 334 B/sample on the headline
+				if (fold && stagger && la == 2) {
+					pass_m = t_batch / 2;
+					if (const char *e = getenv("DSP_B200_FIR_PASS")) pass_m = atoi(e);
+					if (pass_m < 0 || pass_m >= t_batch) pass_m = 0;
+				}
 				// staggered classes of up to 4 adjacent channels (a cluster's four when there are enough channels for every
 				// class to have a whole group): all CTAs of a cluster sum the same partitions, and a cluster that finishes
 				// early hands its SMs to the queued batch CTAs at once instead of waiting for its slowest channel
@@ -2045,10 +2093,18 @@ struct FirOp : Op {
 			const int w = class_w;
 			const int period = T / K;
 			if (q % period != 0) continue;
+			auto class_rows = [&](int c) {
+				int n = 0;
+				for (int G = c; G * w < n_sel; G += K) n += (n_sel - G * w < w) ? n_sel - G * w : w;
+				return n;
+			};
 			const int g = (int) ((q / period) % K);
-			if (n_sel <= g * w) continue;
-			int n_y = 0;   // channels of class g
-			for (int G = g; G * w < n_sel; G += K) n_y += (n_sel - G * w < w) ? n_sel - G * w : w;
+			const int n_y = class_rows(g);
+			// the near tier's grid also holds the mid-window pass of the class whose tier launch came pass_m blocks ago
+			const bool pass = i == 0 && pass_m > 0 && q >= pass_m;
+			const int gp = pass ? (int) ((q - pass_m) % K) : 0;
+			const int n_py = pass ? class_rows(gp) : 0;
+			if (n_y + n_py == 0) continue;
 			if (!any && !serial) CUDA_TRY(cudaStreamWaitEvent(bs, ev_main, 0), return -1);
 			any = true;
 			MacBatchArgs b = {};
@@ -2060,10 +2116,11 @@ struct FirOp : Op {
 			b.p_hi = (i == 0 && t_far > 0) ? t_far + 2 + far_e : L.P;
 			if (i == 0 && t_far > 0) { b.Vin = d_V2; b.vin_slots = 2 * t_far; }
 			b.g = g; b.K = K; b.w = w;
+			if (n_py > 0) { b.n_tier_y = n_y; b.pass_g = gp; b.pass_m = pass_m; }
 			int threads = batch_threads_for(T);
 			if ((batch_threads == 128 || batch_threads == 64) && batch_threads < threads) threads = batch_threads;
 			if (L.B < threads) threads = L.B;
-			dim3 grid(L.B / threads, n_y);
+			dim3 grid(L.B / threads, n_y + n_py);
 			// whole launches of the far tier: at most one CTA per SM (DSP_B200_FIR_FAR_SMEM_KB, 0 = no cap)
 			static const long far_kb = getenv("DSP_B200_FIR_FAR_SMEM_KB") ? atol(getenv("DSP_B200_FIR_FAR_SMEM_KB")) : 0;
 			launch_mac_batch(T, fc == 1, grid, threads, bs, b, i ? "fir_mac_batch_far" : "fir_mac_batch",
@@ -2338,7 +2395,7 @@ struct FirOp : Op {
 							f.init = d_V + (size_t) (L0.blk % (2 * t_batch)) * n_sel * B0;
 						}
 						f.blk = L0.blk;
-						f.cls_T = t_batch; f.cls_K = stagger ? t_batch : 1; f.cls_w = class_w; f.la = la;
+						f.cls_T = t_batch; f.cls_K = stagger ? t_batch : 1; f.cls_w = class_w; f.la = la; f.pass_m = pass_m;
 					}
 					else if (tail_pf == 2 && L0.blk >= 2) {
 						// Y of this block was launched two blocks ago (advance_tail0)
