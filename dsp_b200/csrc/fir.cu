@@ -32,7 +32,7 @@
 //                       register window: every FDL and filter row is read once per T outputs); folded, the near
 //                       tier also takes every partition p < pf+T whose block is complete (the triangle p >= la+t);
 //                       on the full-wave plan the same grid runs the mid-window pass of the class launched m blocks
-//                       earlier, which adds partitions la+t-m .. la-1+t to its periods t >= m (FirOp::pass_m)
+//                       earlier, which adds partitions la+t-m .. la-1+t to its periods t >= m (FirSchedule::pass_m)
 //   k_fir_mac_bulk<8>   calls that bring several whole 8192-blocks: all partitions of up to 8 new blocks in
 //                       one pass, with one forward and one inverse launch (k_fir_fwd / k_fir_inv, gridDim.y)
 //   k_fir_stash/unstash interleaved <-> per-channel copies for multi-level plans and ragged calls
@@ -52,6 +52,7 @@
 #include "common.cuh"
 #include "fft.cuh"
 #include "fir_pipe.cuh"
+#include "fir_plan.h"
 #include "ops.h"
 #include <cooperative_groups.h>
 
@@ -59,8 +60,8 @@ namespace dspb200 {
 
 std::atomic<int> g_fir_serialize{0};   // dspb200_debug_serialize(): no side streams (isolated kernel timings)
 
-constexpr int FIR_MAX_LEVELS = 8;
-constexpr int FIR_MAX_B = 8192;
+template <int... N> constexpr bool fft_cpb_matches() { return ((fir_fft_cpb(N) == FftCfg<N>::CPB) && ...); }
+static_assert(fft_cpb_matches<64, 128, 256, 512, 1024, 2048, 4096, 8192>(), "fir_plan.h's fir_fft_cpb() is FftCfg<N>::CPB");
 
 // ------------------------------------------------------------------------------------------
 // kernels
@@ -1034,12 +1035,6 @@ __global__ void __launch_bounds__(256, FIR_MAC_MINB) k_fir_tail(TailArgs a)
 	}
 }
 
-constexpr int FIR_T_BATCH = 4;   // default depth of the near tier; DSP_B200_FIR_T=4|6|8|12 selects an instantiation
-constexpr int FIR_T_FULL_WAVE = 8;   // ... on full-wave plans (FirOp::plan) of at least 2 * 8 + 3 partitions
-constexpr int FIR_T_FAR = 8;      // default depth of the far tier (DSP_B200_FIR_T2=0|8|12|16) ...
-constexpr int FIR_FAR_MIN_P = 48; // ... on levels of at least this many partitions
-
-static bool batch_depth_ok(int T) { return T == 4 || T == 6 || T == 8 || T == 12 || T == 16; }
 static int batch_threads_for(int T)
 {
 	return (T == 16) ? MacBatchCfg<16>::THREADS : (T == 12) ? MacBatchCfg<12>::THREADS : (T == 8) ? MacBatchCfg<8>::THREADS
@@ -1083,7 +1078,6 @@ static void launch_mac_batch(int T, bool shared_h, dim3 grid, int threads, cudaS
 // `dsp -b 65536`): Y_i = sum_{p<P} X_{j+i-p} H_p for the nb <= T new blocks i in ONE pass -- every FDL row
 // (P + T - 1 of them) and every filter row is streamed once for T outputs, the filter rows slide through a
 // T-deep register window.  Outputs i >= nb are computed on rows that do not exist yet and dropped.
-constexpr int FIR_NB_MAX = 8;
 
 struct MacBulkArgs {
 	const double2 *fdl;   // [s][rows][N]
@@ -1340,8 +1334,6 @@ static int launch_pipe(int N, const PipeArgs &a, cudaStream_t st)
 	}
 }
 
-static bool pipe_size_ok(int N) { return N == 2048 || N == 4096; }
-
 #define DISPATCH_N(N_, FN, ...)                      \
 	switch (N_) {                                    \
 	case 64: return FN<64>(__VA_ARGS__);             \
@@ -1414,21 +1406,10 @@ int test_irfft(int B, int n_ch, const double *d_spec, double *d_out2B, cudaStrea
 // operator
 // ------------------------------------------------------------------------------------------
 struct FirLevel {
-	int B = 0, P = 0;
-	int R = 0;                    // rows of the FDL ring per channel (P, or more when calls bring several blocks at once)
-	long tap0 = 0, tap1 = 0;      // taps [tap0, tap1) of the filter
 	const double2 *tw = nullptr, *ptw = nullptr;
 	double2 *fdl = nullptr, *H = nullptr;
 	double *carry = nullptr, *pend = nullptr;
-	// last level only: partitions p >= 1 ("tail") are summed by the MAC kernels on a side stream, one block
-	// period ahead, into a spectrum that the level's partition-0 kernel adds before its inverse transform
-	bool tail = false;
 	long blk = 0;                 // completed blocks of this level
-
-	void free_all()
-	{
-		dev_free(fdl); dev_free(H); dev_free(carry); dev_free(pend);
-	}
 };
 
 struct FirOp : Op {
@@ -1440,23 +1421,18 @@ struct FirOp : Op {
 	long latency = 0;
 	int n_sel = 0;
 	bool multilevel = true;
+	bool direct_io = !(getenv("DSP_B200_FIR_NO_DIRECT") && getenv("DSP_B200_FIR_NO_DIRECT")[0] == '1');
 
-	// plan
+	// plan (fir_plan.h) and, per level, what it allocated
 	bool planned = false;
-	int B0 = 0, n_levels = 0;
+	FirSchedule s;
 	FirLevel lv[FIR_MAX_LEVELS];
-	long hist_len = 0;
 
 	// device state
 	int *d_ch_map = nullptr;
 	double *d_hist = nullptr, *d_ytmp = nullptr, *d_pre = nullptr, *d_h0 = nullptr;
 	double2 *d_Y = nullptr;              // [n_sel][max B]
 	double2 *d_Y_side = nullptr;         // [n_sel][B last]: the tail spectrum of the next block period (side stream); two of them when level 0 has the tail
-	int tail_pf = 0;                     // 0: no tail; 1: tail on an upper level; 2: tail on level 0 (single-level plan, fused kernel sums p = 0, 1)
-	// single-level plans of 2048/4096-frame blocks: whole aligned blocks go through the persistent pipeline
-	// (fir_pipe.cuh), which sums partitions 0 .. pipe_pf-1 (+ the batched V) itself -- no per-block k_fir_mac
-	bool use_pipe = false;
-	int pipe_pf = 0;
 	int pipe_evict_first = getenv("DSP_B200_FIR_PIPE_EVICT") ? atoi(getenv("DSP_B200_FIR_PIPE_EVICT")) : 1;
 	int pipe_fake_io = getenv("DSP_B200_FIR_PIPE_FAKEIO") ? atoi(getenv("DSP_B200_FIR_PIPE_FAKEIO")) : 0;   // measurement only
 	int pipe_no_items = getenv("DSP_B200_FIR_PIPE_NOITEMS") ? atoi(getenv("DSP_B200_FIR_PIPE_NOITEMS")) : 0;   // measurement only
@@ -1468,71 +1444,19 @@ struct FirOp : Op {
 	// side stream: the upper levels' partition-0 kernels and the last level's tail MAC overlap the main stream
 	cudaStream_t side = nullptr;
 	cudaEvent_t ev_main = nullptr, ev_urgent = nullptr;
-	// time-batched tail (see k_fir_mac_batch): V spectra for 2 T block periods, produced T at a time on a second side stream
-	int t_batch = 0;
-	double2 *d_V = nullptr;
+	// batch tiers: V spectra of the near tier (2 t_batch block periods) and of the far tier (2 t_far), on a second side stream
+	double2 *d_V = nullptr, *d_V2 = nullptr;
 	cudaStream_t side2 = nullptr;
 	cudaEvent_t ev_batch[2] = { nullptr, nullptr };
-	// single-level plans: a second, deeper tier over the oldest partitions (its sums are the near tier's starting
-	// value), and the staggered schedule -- every block launches the tiers for the channels of one residue class
-	// (s mod T == block mod T) instead of all channels every T-th block, so that every block period carries the same work
-	int t_far = 0;
-	// The far tier works one near-tier period ahead: launched after block q it covers the periods q+3+far_e .. (it takes
-	// partitions >= t_far + 2 + far_e), so that the near-tier launch that starts from its sums comes far_e blocks later.
-	// Without it a whole-launch far tier sits between a block and the third block after it: the step time then depends
-	// on how fast that one launch happens to run.
-	int far_e = 0;
-	// Far tier in whole launches: far_classes residue classes of channels take turns, one launch every t_far /
-	// far_classes blocks (DSP_B200_FIR_FAR_CLASSES=2: half the channels every fourth block at t_far = 8)
-	int far_classes = 1;
-	bool merge_tail = false;             // the per-block MAC and the staggered batch launch as one grid (k_fir_tail)
-	double2 *d_V2 = nullptr;             // far tier: V spectra for 2 t_far block periods
-	bool stagger = false;
 	cudaEvent_t ev_bs[8] = {};           // after the tier launches of a block (ring), ev_bs_last: the latest one
 	int ev_bs_n = 0;
 	cudaEvent_t ev_bs_last = nullptr;
-	// folded tail: the fused kernel of block j starts from V_j, which the tier launches up to block j-la complete;
-	// ev_bs_at[q & 3] = ev_bs_last as it was after block q
-	bool fold = false;
-	cudaEvent_t ev_bs_at[4] = {};
-	// look-ahead of the folded near tier: its launch after block q covers the periods q+la .. q+la+T-1, from partition
-	// la + t on for period q+la+t (every block involved is complete).  3 by default; 2 on the full-wave plan (below),
-	// where the fused kernel is the step's critical path and one partition fewer per block shortens it.
-	// Invariants (T = t_batch):
-	//  - the V ring of 2 T slots is safe for T >= la: the next write to V_j's slot is for period j + 2T, by a launch after
-	//    block j + T - la + 1 > j or later, and launches only start once the fused kernel of their block is complete;
-	//  - FDL row j mod P (X_{j-P} until block j overwrites it) is read by the tier launches after blocks up to j-la-1;
-	//    the fused kernel of block j waits for the launches up to j-la, which covers them;
-	//  - the general path (wait_batch_for) still waits for every launch made so far.
-	int la = 3;
-	// mid-window pass (staggered full-wave plans with one tier, la = 2; DSP_B200_FIR_PASS=0|m, default T/2): the grid
-	// launched after block q' also runs a pass for the class whose tier launch came after block q = q' - pass_m.  For
-	// its periods q+la+t with t >= pass_m it adds partitions la+t-pass_m .. la-1+t to V in place (blocks q'-pass_m+1 ..
-	// q'), and the fused kernel sums 0 .. la-1+t-pass_m there: la .. la-1+max(pass_m, T-pass_m) partitions instead of
-	// la .. la-1+T.  Invariants, in addition to those of `la`:
-	//  - the pass after q' reads X_{q'} and waits for the fused kernel of block q', like the tier launch after q';
-	//  - the fused kernel of block j = q+la+t, t >= pass_m, waits for the launches up to j-la = q+t >= q', the pass included;
-	//  - V slots: the pass touches the periods q+la+pass_m .. q+la+T-1; the class's next tier launch (after q+T) writes
-	//    q+T+la .. q+2T+la-1: disjoint in the ring of 2T slots; their next writer, the tier launch after q+2T, comes after
-	//    the fused kernels that read them;
-	//  - FDL: the pass reads only rows newer than the tier launch of the same grid does (q'-pass_m+1 .. q'); the first
-	//    block to overwrite one, q'-pass_m+1+P, waits for the launches up to q'-pass_m+1+P-la >= q' (P >= 2T+3).
-	int pass_m = 0;
-	// staggered folded plans: the classes take turns over groups of class_w adjacent channels (1 otherwise), so that
-	// the four channels of a cluster sum the same number of partitions and finish together
-	int class_w = 1;
+	cudaEvent_t ev_bs_at[4] = {};        // folded: ev_bs_at[q & 3] = ev_bs_last as it was after block q
 	cudaEvent_t ev_join[2] = { nullptr, nullptr };
-	// single-level tail plans: the fused kernel of every block goes to a stream of the highest priority (the caller's
-	// stream hands over and takes back with two events): its CTAs are placed before the queued CTAs of the
-	// look-ahead MACs, which share the lowest priority with a caller's default stream otherwise
-	cudaStream_t hot = nullptr;
+	cudaStream_t hot = nullptr;          // FirSchedule::hot
 	cudaEvent_t ev_hot_in = nullptr, ev_hot_out = nullptr;
 	bool urgent_pending = false;
 	long ltmp_cap = 0;
-	// bulk form (single-level plans): up to nb_max whole blocks of one call are transformed, multiplied and
-	// overlapped by one launch each
-	int nb_max = 1;
-	bool direct_io = !(getenv("DSP_B200_FIR_NO_DIRECT") && getenv("DSP_B200_FIR_NO_DIRECT")[0] == '1');
 	bool cluster_ok = false;   // selected channels are contiguous, start on an even channel, and come in fours
 	double2 *d_Ybulk = nullptr;
 	double *d_lo = nullptr, *d_hi = nullptr;
@@ -1545,74 +1469,31 @@ struct FirOp : Op {
 
 	const char *name() const override { return "fir"; }
 
-	// partitions level 0's fused kernel sums on whole aligned blocks: at most, and (folded: once every class has had a
-	// near-tier launch) at least
-	int l0_parts() const { return fold ? t_batch + la - 1 : (lv[0].P < 2) ? lv[0].P : 2; }
-	int l0_parts_min() const { return fold ? la : l0_parts(); }
-	// at most, once every class has had its mid-window pass (l0_parts() without one)
-	int l0_parts_steady() const { return fold ? la - 1 + ((pass_m > t_batch - pass_m) ? pass_m : t_batch - pass_m) : l0_parts(); }
-
 	std::string describe() const override
 	{
 		char buf[1024];
-		int n = snprintf(buf, sizeof(buf), "{\"op\":\"fir\",\"taps\":%ld,\"n_sel\":%d,\"filter_channels\":%d,\"latency\":%ld,\"planned\":%d,\"levels\":[",
-		                 filter_frames, n_sel, fc, latency, planned ? 1 : 0);
-		for (int l = 0; l < n_levels && n < (int) sizeof(buf) - 64; ++l)
-			n += snprintf(buf + n, sizeof(buf) - n, "%s{\"B\":%d,\"P\":%d}", l ? "," : "", lv[l].B, lv[l].P);
-		n += snprintf(buf + n, sizeof(buf) - n, "],\"t_batch\":%d,\"t_far\":%d,\"far_e\":%d,\"far_classes\":%d,\"stagger\":%d,\"class_width\":%d,\"merge\":%d,\"tail_pf\":%d,"
-		              "\"l0_parts\":%d,\"l0_parts_min\":%d,\"l0_parts_steady\":%d,\"lookahead\":%d,\"pass_m\":%d,\"bulk\":%d,\"pipe\":%d,\"pipe_pf\":%d,",
-		              t_batch, t_far, far_e, far_classes, stagger ? 1 : 0, class_w, merge_tail ? 1 : 0, tail_pf, l0_parts(), l0_parts_min(),
-		              l0_parts_steady(), la, pass_m, nb_max, use_pipe ? 1 : 0, pipe_pf);
-		snprintf(buf + n, sizeof(buf) - n, "\"replans\":%d,\"paths\":{\"fused\":%ld,\"cluster\":%ld,\"pipe\":%ld,\"bulk\":%ld,\"general\":%ld,\"head\":%ld}}",
-		         replans, n_fused, n_cluster, n_pipe, n_bulk, n_general, n_head);
+		snprintf(buf, sizeof(buf), "{\"op\":\"fir\",\"taps\":%ld,\"n_sel\":%d,\"filter_channels\":%d,\"latency\":%ld,\"planned\":%d,%s,"
+		         "\"replans\":%d,\"paths\":{\"fused\":%ld,\"cluster\":%ld,\"pipe\":%ld,\"bulk\":%ld,\"general\":%ld,\"head\":%ld}}",
+		         filter_frames, n_sel, fc, latency, planned ? 1 : 0, fir_schedule_json(s).c_str(), replans, n_fused, n_cluster, n_pipe, n_bulk,
+		         n_general, n_head);
 		return buf;
 	}
 
 	// everything plan() made: streams, events, spectra, work buffers (the description, d_ch_map and the host taps stay)
 	void free_plan()
 	{
-		if (side) {
-			cudaStreamSynchronize(side);
-			cudaStreamDestroy(side);
-			side = nullptr;
-		}
-		if (side2) {
-			cudaStreamSynchronize(side2);
-			cudaStreamDestroy(side2);
-			side2 = nullptr;
-		}
-		if (hot) {
-			cudaStreamSynchronize(hot);
-			cudaStreamDestroy(hot);
-			hot = nullptr;
-		}
-		if (ev_hot_in) cudaEventDestroy(ev_hot_in);
-		if (ev_hot_out) cudaEventDestroy(ev_hot_out);
-		ev_hot_in = ev_hot_out = nullptr;
-		for (cudaEvent_t &e : ev_batch) { if (e) cudaEventDestroy(e); e = nullptr; }
+		for (cudaStream_t *q : { &side, &side2, &hot })
+			if (*q) { cudaStreamSynchronize(*q); cudaStreamDestroy(*q); *q = nullptr; }
+		for (cudaEvent_t *e : { &ev_hot_in, &ev_hot_out, &ev_batch[0], &ev_batch[1], &ev_tail[0], &ev_tail[1], &ev_join[0], &ev_join[1], &ev_main, &ev_urgent })
+			if (*e) { cudaEventDestroy(*e); *e = nullptr; }
 		for (cudaEvent_t &e : ev_bs) { if (e) cudaEventDestroy(e); e = nullptr; }
-		ev_bs_last = nullptr; ev_bs_n = 0;
-		for (cudaEvent_t &e : ev_bs_at) e = nullptr;
-		fold = false;
-		la = 3;
-		pass_m = 0;
-		class_w = 1;
-		for (cudaEvent_t &e : ev_tail) { if (e) cudaEventDestroy(e); e = nullptr; }
-		for (cudaEvent_t &e : ev_join) { if (e) cudaEventDestroy(e); e = nullptr; }
-		if (ev_main) cudaEventDestroy(ev_main);
-		if (ev_urgent) cudaEventDestroy(ev_urgent);
-		ev_main = ev_urgent = nullptr;
-		for (int l = 0; l < n_levels; ++l) {
-			lv[l].free_all();
-			lv[l] = FirLevel();
-		}
-		n_levels = 0;
+		ev_bs_last = nullptr; ev_bs_n = 0; for (cudaEvent_t &e : ev_bs_at) e = nullptr;
+		for (FirLevel &L : lv) { dev_free(L.fdl); dev_free(L.H); dev_free(L.carry); dev_free(L.pend); L = FirLevel(); }
 		dev_free(d_V); dev_free(d_V2); dev_free(d_Y_side); dev_free(d_hist); dev_free(d_ytmp); dev_free(d_pre); dev_free(d_h0);
 		dev_free(d_Y); dev_free(d_ring); dev_free(d_ltmp); dev_free(d_Ybulk); dev_free(d_lo); dev_free(d_hi); dev_free(d_stats);
-		d_V = d_V2 = d_Y_side = nullptr; t_far = 0; far_e = 0; far_classes = 1; stagger = false; merge_tail = false; d_hist = d_ytmp = d_pre = d_h0 = nullptr; d_Y = nullptr; d_ring = d_ltmp = nullptr;
-		d_Ybulk = nullptr; d_lo = d_hi = nullptr; d_stats = nullptr;
-		ltmp_cap = 0; tail_pf = 0; t_batch = 0; use_pipe = false; pipe_pf = 0; nb_max = 1;
-		urgent_pending = false; pre_valid = false; abs_pos = 0; planned = false;
+		d_V = d_V2 = d_Y_side = d_Y = d_Ybulk = nullptr; d_hist = d_ytmp = d_pre = d_h0 = d_ring = d_ltmp = d_lo = d_hi = nullptr; d_stats = nullptr;
+		ltmp_cap = 0; urgent_pending = false; pre_valid = false; abs_pos = 0; planned = false;
+		s = FirSchedule{};
 	}
 
 	~FirOp() override
@@ -1622,202 +1503,61 @@ struct FirOp : Op {
 		dev_free(d_replay);
 	}
 
+	// the schedule fir_schedule() picks for calls of `hint` frames, then what it needs: spectra, rings, streams, events
 	int plan(long hint, cudaStream_t st)
 	{
-		int b = 64;
-		while (b * 2 <= hint && b < FIR_MAX_B) b *= 2;
-		B0 = b;
+		const FirKnobs k = FirKnobs::from_env();
+		s = fir_schedule({ filter_frames, hint, n_sel, sm_count(), multilevel, direct_io }, k);
 		n_fused = n_cluster = n_pipe = n_bulk = n_general = n_head = 0;
 		const long T = filter_frames;
-		// level plan (see the header comment)
-		n_levels = 0;
-		// Partitions grow up to `cap`: beyond it the larger transforms (one CTA per SM, twice the passes) cost
-		// more than the filter traffic they save once the tail is time-batched (measured, DESIGN.md K2)
-		long cap = 4096;
-		if (const char *e = getenv("DSP_B200_FIR_LEVEL_CAP")) cap = atol(e);
-		if (cap < B0) cap = B0;
-		if (cap > FIR_MAX_B) cap = FIR_MAX_B;
-		// Blocks of 2048 frames stay a single level of 2048-frame partitions: with the two-tier batched tail it moves
-		// fewer bytes per sample than 2048 + 4096 (544 against 612 at 131072 taps) and every block period carries the
-		// same kernels (no upper-level kernel that has to land between two blocks)
-		long single_min = 2048;
-		if (const char *e = getenv("DSP_B200_FIR_SINGLE_MIN")) single_min = atol(e);
-		if (!multilevel || T <= 2L * B0 || B0 >= cap || B0 >= single_min) {
-			lv[0].B = B0; lv[0].tap0 = 0; lv[0].tap1 = T;
-			n_levels = 1;
-		}
-		else {
-			lv[0].B = B0; lv[0].tap0 = 0; lv[0].tap1 = 2L * B0;
-			n_levels = 1;
-			long B = 2L * B0;
-			while (n_levels < FIR_MAX_LEVELS) {
-				FirLevel &L = lv[n_levels++];
-				L.B = (int) B; L.tap0 = B;
-				if (B >= cap || T <= 2 * B || n_levels == FIR_MAX_LEVELS) { L.tap1 = T; break; }
-				L.tap1 = 2 * B;
-				B *= 2;
-			}
-		}
 		const int nh = (fc == 1) ? 1 : n_sel;
-		int Bmax = 0;
-		for (int l = 0; l < n_levels; ++l) {
+		for (int l = 0; l < s.n_levels; ++l) {
 			FirLevel &L = lv[l];
-			L.P = (int) ((L.tap1 - L.tap0 + L.B - 1) / L.B);
-			L.R = L.P;
-			if (n_levels == 1 && L.P > 2 && hint >= 2L * L.B && !(getenv("DSP_B200_FIR_NO_BULK") && getenv("DSP_B200_FIR_NO_BULK")[0] == '1')) {
-				nb_max = (int) ((hint / L.B < FIR_NB_MAX) ? hint / L.B : FIR_NB_MAX);
-				L.R = L.P + nb_max - 1;
-			}
-			L.tw = twiddles_2n(L.B);
-			L.ptw = twiddles_pass(L.B);
+			const FirLevelPlan &Lp = s.lv[l];
+			L.tw = twiddles_2n(Lp.B);
+			L.ptw = twiddles_pass(Lp.B);
 			if (!L.tw || !L.ptw) return -1;
-			L.fdl = dev_alloc<double2>((size_t) n_sel * L.R * L.B);
-			L.H = dev_alloc<double2>((size_t) nh * L.P * L.B);
-			L.carry = dev_alloc<double>((size_t) n_sel * L.B);
-			if (l > 0) L.pend = dev_alloc<double>((size_t) n_sel * L.B);
+			L.fdl = dev_alloc<double2>((size_t) n_sel * Lp.R * Lp.B);
+			L.H = dev_alloc<double2>((size_t) nh * Lp.P * Lp.B);
+			L.carry = dev_alloc<double>((size_t) n_sel * Lp.B);
+			if (l > 0) L.pend = dev_alloc<double>((size_t) n_sel * Lp.B);
 			if (!L.fdl || !L.H || !L.carry || (l > 0 && !L.pend)) return -1;
-			// the last level's partitions beyond those its fused kernel sums form the "tail"; a single level keeps
-			// partitions 0 and 1 in the kernel (pf = 2), an upper level only partition 0 (pf = 1)
-			const int pf = (l == 0) ? 2 : 1;
-			const bool has_tail = (l == n_levels - 1) && L.P > pf && (l > 0 || (nb_max == 1 && multilevel));
-			if ((l > 0 || has_tail) && !side) {
-				int lo = 0, hi = 0;
-				cudaDeviceGetStreamPriorityRange(&lo, &hi);
-				// multi-level plans: the side stream carries the upper levels' block kernels, whose result the caller's
-				// stream waits for at its next block -- they must not queue behind the batched MAC's CTAs (otherwise
-				// the step time depends on who gets the SMs first).  Single-level
-				// plans only keep look-ahead MACs there: lowest priority.
-				// (DSP_B200_FIR_MAC_PRIO: measurement -- the per-block MAC between the fused kernel and the batch tiers)
-				int side_prio = (n_levels > 1) ? hi : lo;
-				if (const char *e = getenv("DSP_B200_FIR_MAC_PRIO")) side_prio = (atoi(e) < hi) ? hi : (atoi(e) > lo) ? lo : atoi(e);
-				CUDA_TRY(cudaStreamCreateWithPriority(&side, cudaStreamNonBlocking, side_prio), return -1);
-				CUDA_TRY(cudaEventCreateWithFlags(&ev_main, cudaEventDisableTiming), return -1);
-				CUDA_TRY(cudaEventCreateWithFlags(&ev_urgent, cudaEventDisableTiming), return -1);
-			}
-			if (has_tail) {
-				L.tail = true;
-				tail_pf = pf;
-				// the one-kernel-per-block pipeline (fir_pipe.cuh) is opt-in: slower than the three-kernel step on the
-				// headline (DESIGN.md K2), it stays selectable for measurements and is covered by the tests
-				const char *pe = getenv("DSP_B200_FIR_PIPE");
-				use_pipe = (l == 0) && direct_io && pipe_size_ok(L.B) && (pe && pe[0] == '1');
-				const char *he = getenv("DSP_B200_FIR_HOT");
-				if (!use_pipe && l == 0 && direct_io && !(he && he[0] == '0')) {
-					int lo = 0, hi = 0;
-					cudaDeviceGetStreamPriorityRange(&lo, &hi);
-					CUDA_TRY(cudaStreamCreateWithPriority(&hot, cudaStreamNonBlocking, hi), return -1);
-					CUDA_TRY(cudaEventCreateWithFlags(&ev_hot_in, cudaEventDisableTiming), return -1);
-					CUDA_TRY(cudaEventCreateWithFlags(&ev_hot_out, cudaEventDisableTiming), return -1);
-				}
-				// The fold pays once the fused kernel's CTAs outnumber half the SMs (see `fold` below).  Those plans are
-				// "full-wave": the fused kernel fills the GPU and carries most of the bytes, so the near tier goes deeper
-				// (T = 8 reads every FDL and filter row once per 8 periods instead of 4: 440 -> 388 B/sample on the
-				// headline) and, with one tier, looks two blocks ahead instead of three (la = 2: 360 B/sample).
-				const int cpb = (L.B / 16 >= 256) ? 1 : 256 / (L.B / 16);   // FftCfg<B>::CPB
-				const bool fold_pays = 2 * ceil_div(n_sel, cpb) > sm_count();
-				const bool full_wave = l == 0 && !use_pipe && direct_io && fold_pays;
-				const char *nb = getenv("DSP_B200_FIR_NO_BATCH");
-				int tb = (full_wave && L.P >= 2 * FIR_T_FULL_WAVE + pf + 1) ? FIR_T_FULL_WAVE : FIR_T_BATCH;
-				if (const char *e = getenv("DSP_B200_FIR_T")) tb = (atoi(e) == 12) ? 12 : (atoi(e) == 8) ? 8 : (atoi(e) == 6) ? 6 : 4;
-				if (use_pipe) tb = PIPE_TB;   // the pipeline kernel's batch depth is compiled in (one channel residue per block)
-				if (L.P >= 2 * tb + pf + 1 && !(nb && nb[0] == '1')) {
-					t_batch = tb;
-					d_V = dev_alloc<double2>((size_t) 2 * t_batch * n_sel * L.B);
-					if (!d_V) return -1;
-					if (!use_pipe) {
-						int lo = 0, hi = 0;
-						cudaDeviceGetStreamPriorityRange(&lo, &hi);
-						CUDA_TRY(cudaStreamCreateWithPriority(&side2, cudaStreamNonBlocking, lo), return -1);
-						CUDA_TRY(cudaEventCreateWithFlags(&ev_batch[0], cudaEventDisableTiming), return -1);
-						CUDA_TRY(cudaEventCreateWithFlags(&ev_batch[1], cudaEventDisableTiming), return -1);
-					}
-					if (!use_pipe && pf == 2) {
-						// far tier: partitions >= t_far + 2, T = t_far periods per launch; only when the level is long
-						// enough for it to pay (the near tier keeps partitions t_batch + 2 .. t_far + 1)
-						// (at 32 partitions the second tier saves bytes but no time; at 64 partitions -- 2048-frame blocks --
-						// it pays behind a near tier of 4.  On the full-wave plan the near tier of 8 leaves no far tier of
-						// 8: one staggered tier of 8 looking two blocks ahead measured 9% faster than tiers 4 + 8 at 256
-						// channels of 2048 frames, and 5% faster than tiers 8 + 16, DESIGN.md K2)
-						int t2 = (L.P >= FIR_FAR_MIN_P) ? FIR_T_FAR : 0;
-						if (const char *e = getenv("DSP_B200_FIR_T2")) t2 = atoi(e);
-						if (!batch_depth_ok(t2) || t2 <= t_batch || t2 % t_batch != 0 || L.P < 2 * t2 + pf + t_batch) t2 = 0;
-						if (t2 > 0) {
-							t_far = t2;
-							far_e = t_batch;
-							d_V2 = dev_alloc<double2>((size_t) 2 * t_far * n_sel * L.B);
-							if (!d_V2) return -1;
-						}
-						// one tier: staggered (every block period carries the same launches); two tiers: whole launches (the
-						// small per-class launches of the deep tier run at half the efficiency of a whole one)
-						// (and a tail too short for its per-class launches to be worth their overhead: config 5's 16
-						// partitions run faster in whole launches)
-						const char *sg = getenv("DSP_B200_FIR_STAGGER");
-						stagger = sg ? sg[0] != '0' : (t_far == 0 && L.P - t_batch - pf >= 16);
-						if (t_far > 0 && !stagger) {
-							// the turns must start on near-tier launches: t_far / far_classes a multiple of t_batch
-							// (one turn by default: two were no faster on 2048-frame blocks)
-							int fcls = 1;
-							if (const char *e = getenv("DSP_B200_FIR_FAR_CLASSES")) fcls = atoi(e);
-							far_classes = (fcls >= 1 && t_far % fcls == 0 && (t_far / fcls) % t_batch == 0) ? fcls : 1;
-						}
-						const char *mg = getenv("DSP_B200_FIR_MERGE");
-						// (opt-in: alone the one grid streams faster than the two launches, but the fused kernel of the
-						// block after next then waits for all of it instead of the MAC part: a slower step)
-						merge_tail = stagger && t_far == 0 && t_batch == 4 && L.B >= 256 && (mg && mg[0] == '1');
-						for (cudaEvent_t &e : ev_bs) CUDA_TRY(cudaEventCreateWithFlags(&e, cudaEventDisableTiming), return -1);
-					}
-				}
-				if (use_pipe) {
-					pipe_pf = (t_batch > 0) ? t_batch + 2 : L.P;
-					if (getenv("DSP_B200_FIR_PIPE_STATS")) d_stats = dev_alloc<long long>(8 * 1024);
-				}
-				// Folded tail (single level, direct I/O, a batch tier): the fused kernel starts from the near tier's V_j and
-				// sums what that tier leaves out, la .. t_batch+la-1 partitions (launch_tiers0) -- no per-block MAC, no Y
-				// spectrum through HBM (DESIGN.md K2).  Only when the fused kernel's CTAs outnumber half the SMs: with
-				// fewer, the per-block MAC streams on the SMs the fused kernel leaves idle, and moving its partitions into
-				// the few fused CTAs lengthens the step (64 channels of 4096 frames: 8% slower folded, 256: 6% faster).
-				// DSP_B200_FIR_FOLD=1 / 0 force either form (tests, measurements); the merged grid is a per-block MAC.
-				// The look-ahead of 2 is for full-wave plans with one tier only (a far tier keeps 3).
-				const char *fe = getenv("DSP_B200_FIR_FOLD");
-				fold = l == 0 && !use_pipe && direct_io && t_batch > 0 && !merge_tail && (fe ? fe[0] == '1' : fold_pays);
-				la = (fold && full_wave && t_far == 0) ? 2 : 3;
-				// the mid-window pass halves the fused kernel's triangle (see `pass_m`): 360 -> 334 B/sample on the headline
-				if (fold && stagger && la == 2) {
-					pass_m = t_batch / 2;
-					if (const char *e = getenv("DSP_B200_FIR_PASS")) pass_m = atoi(e);
-					if (pass_m < 0 || pass_m >= t_batch) pass_m = 0;
-				}
-				// staggered classes of up to 4 adjacent channels (a cluster's four when there are enough channels for every
-				// class to have a whole group): all CTAs of a cluster sum the same partitions, and a cluster that finishes
-				// early hands its SMs to the queued batch CTAs at once instead of waiting for its slowest channel
-				if (fold && stagger) {
-					const int most = (n_sel / t_batch < 4) ? n_sel / t_batch : 4;
-					while (class_w * 2 <= most) class_w *= 2;
-				}
-				if (!use_pipe && !fold) {
-					d_Y_side = dev_alloc<double2>((size_t) pf * n_sel * L.B);
-					if (!d_Y_side) return -1;
-					if (l == 0) {
-						CUDA_TRY(cudaEventCreateWithFlags(&ev_tail[0], cudaEventDisableTiming), return -1);
-						CUDA_TRY(cudaEventCreateWithFlags(&ev_tail[1], cudaEventDisableTiming), return -1);
-					}
-				}
-			}
-			if (L.B > Bmax) Bmax = L.B;
 		}
-		// upper levels read their block from the ring on the side stream while the next block is already
-		// being stashed: keep two of the largest blocks
-		hist_len = (n_levels > 1) ? 2L * Bmax : (long) nb_max * Bmax;
-		if (nb_max > 1) {
-			d_Ybulk = dev_alloc<double2>((size_t) nb_max * n_sel * B0, false);
-			d_lo = dev_alloc<double>((size_t) nb_max * n_sel * B0, false);
-			d_hi = dev_alloc<double>((size_t) nb_max * n_sel * B0, false);
+		auto stream = [](cudaStream_t &q, int prio) { CUDA_TRY(cudaStreamCreateWithPriority(&q, cudaStreamNonBlocking, prio), return false); return true; };
+		auto events = [](std::initializer_list<cudaEvent_t *> es) { for (cudaEvent_t *e : es) CUDA_TRY(cudaEventCreateWithFlags(e, cudaEventDisableTiming), return false); return true; };
+		const size_t rows = (size_t) n_sel * s.lv[s.n_levels - 1].B;
+		int lo = 0, hi = 0;
+		cudaDeviceGetStreamPriorityRange(&lo, &hi);
+		if (s.n_levels > 1 || s.tail_pf > 0) {
+			// multi-level plans: the side stream carries the upper levels' block kernels, which must not queue behind the
+			// batched MAC's CTAs; single-level plans only keep look-ahead MACs there: lowest priority.
+			// (DSP_B200_FIR_MAC_PRIO: measurement -- the per-block MAC between the fused kernel and the batch tiers)
+			int side_prio = (s.n_levels > 1) ? hi : lo;
+			if (k.mac_prio) side_prio = (*k.mac_prio < hi) ? hi : (*k.mac_prio > lo) ? lo : *k.mac_prio;
+			if (!stream(side, side_prio) || !events({ &ev_main, &ev_urgent })) return -1;
+		}
+		if (s.hot && (!stream(hot, hi) || !events({ &ev_hot_in, &ev_hot_out }))) return -1;
+		if (s.t_batch > 0 && !(d_V = dev_alloc<double2>(2 * s.t_batch * rows))) return -1;
+		if (s.t_batch > 0 && !s.use_pipe && (!stream(side2, lo) || !events({ &ev_batch[0], &ev_batch[1] }))) return -1;
+		if (s.t_far > 0 && !(d_V2 = dev_alloc<double2>(2 * s.t_far * rows))) return -1;
+		if (s.t_batch > 0 && !s.use_pipe && s.tail_pf == 2)
+			for (cudaEvent_t &e : ev_bs) if (!events({ &e })) return -1;
+		if (s.use_pipe && k.pipe_stats) d_stats = dev_alloc<long long>(8 * 1024);
+		if (s.tail_pf > 0 && !s.use_pipe && !s.fold) {
+			if (!(d_Y_side = dev_alloc<double2>(s.tail_pf * rows))) return -1;
+			if (s.tail_pf == 2 && !events({ &ev_tail[0], &ev_tail[1] })) return -1;
+		}
+		const int B0 = s.B0;
+		if (s.nb_max > 1) {
+			d_Ybulk = dev_alloc<double2>((size_t) s.nb_max * n_sel * B0, false);
+			d_lo = dev_alloc<double>((size_t) s.nb_max * n_sel * B0, false);
+			d_hi = dev_alloc<double>((size_t) s.nb_max * n_sel * B0, false);
 			if (!d_Ybulk || !d_lo || !d_hi) return -1;
 		}
-		d_hist = dev_alloc<double>((size_t) n_sel * hist_len);
+		d_hist = dev_alloc<double>((size_t) n_sel * s.hist_len);
 		d_ytmp = dev_alloc<double>((size_t) n_sel * B0);
 		d_pre = dev_alloc<double>((size_t) n_sel * B0);
-		d_Y = dev_alloc<double2>((size_t) n_sel * Bmax);
+		d_Y = dev_alloc<double2>((size_t) n_sel * s.Bmax);
 		d_h0 = dev_alloc<double>((size_t) nh * B0);
 		if (latency > 0) d_ring = dev_alloc<double>((size_t) latency * n_sel);
 		if (!d_hist || !d_ytmp || !d_pre || !d_Y || !d_h0 || (latency > 0 && !d_ring)) return -1;
@@ -1826,16 +1566,16 @@ struct FirOp : Op {
 		double *d_taps = dev_alloc<double>((size_t) nh * T, false);
 		if (!d_taps) return -1;
 		CUDA_TRY(cudaMemcpyAsync(d_taps, h_taps.data(), (size_t) nh * T * sizeof(double), cudaMemcpyHostToDevice, st), return -1);
-		for (int l = 0; l < n_levels; ++l) {
-			FirLevel &L = lv[l];
-			for (int p = 0; p < L.P; ++p) {
+		for (int l = 0; l < s.n_levels; ++l) {
+			const FirLevelPlan &Lp = s.lv[l];
+			for (int p = 0; p < Lp.P; ++p) {
 				FwdArgs a = {};
-				const long t0 = L.tap0 + (long) p * L.B;
+				const long t0 = Lp.tap0 + (long) p * Lp.B;
 				a.in = d_taps + t0; a.ch_stride = T;
-				a.valid = L.tap1 - t0;
-				if (a.valid > L.B) a.valid = L.B;
-				a.spec = L.H; a.spec_ch_stride = (long) L.P * L.B; a.slot = p; a.tw = L.tw; a.ptw = L.ptw; a.n_ch = nh;
-				if (launch_fwd(L.B, a, st)) return -1;
+				a.valid = Lp.tap1 - t0;
+				if (a.valid > Lp.B) a.valid = Lp.B;
+				a.spec = lv[l].H; a.spec_ch_stride = (long) Lp.P * Lp.B; a.slot = p; a.tw = lv[l].tw; a.ptw = lv[l].ptw; a.n_ch = nh;
+				if (launch_fwd(Lp.B, a, st)) return -1;
 			}
 		}
 		// time-domain head taps h0[c][0:B0)
@@ -1878,43 +1618,48 @@ struct FirOp : Op {
 		if (!planned) return;
 		if (side) cudaStreamSynchronize(side);
 		if (side2) cudaStreamSynchronize(side2);
-		if (d_V) cudaMemsetAsync(d_V, 0, (size_t) 2 * t_batch * n_sel * lv[n_levels - 1].B * sizeof(double2), st);
-		if (d_V2) cudaMemsetAsync(d_V2, 0, (size_t) 2 * t_far * n_sel * lv[n_levels - 1].B * sizeof(double2), st);
+		if (d_V) cudaMemsetAsync(d_V, 0, (size_t) 2 * s.t_batch * n_sel * s.lv[s.n_levels - 1].B * sizeof(double2), st);
+		if (d_V2) cudaMemsetAsync(d_V2, 0, (size_t) 2 * s.t_far * n_sel * s.lv[s.n_levels - 1].B * sizeof(double2), st);
 		ev_bs_last = nullptr;
 		for (cudaEvent_t &e : ev_bs_at) e = nullptr;
-		for (int l = 0; l < n_levels; ++l) {
+		for (int l = 0; l < s.n_levels; ++l) {
 			FirLevel &L = lv[l];
+			const FirLevelPlan &Lp = s.lv[l];
 			L.blk = 0;
-			cudaMemsetAsync(L.fdl, 0, (size_t) n_sel * L.R * L.B * sizeof(double2), st);
-			cudaMemsetAsync(L.carry, 0, (size_t) n_sel * L.B * sizeof(double), st);
-			if (L.pend) cudaMemsetAsync(L.pend, 0, (size_t) n_sel * L.B * sizeof(double), st);
+			cudaMemsetAsync(L.fdl, 0, (size_t) n_sel * Lp.R * Lp.B * sizeof(double2), st);
+			cudaMemsetAsync(L.carry, 0, (size_t) n_sel * Lp.B * sizeof(double), st);
+			if (L.pend) cudaMemsetAsync(L.pend, 0, (size_t) n_sel * Lp.B * sizeof(double), st);
 		}
-		cudaMemsetAsync(d_hist, 0, (size_t) n_sel * hist_len * sizeof(double), st);
+		cudaMemsetAsync(d_hist, 0, (size_t) n_sel * s.hist_len * sizeof(double), st);
 		if (d_ring) cudaMemsetAsync(d_ring, 0, (size_t) latency * n_sel * sizeof(double), st);
 	}
 
-	void mac(FirLevel &L, int p0, int p1, long slot_blk, cudaStream_t st, double2 *Y = nullptr, const double2 *init = nullptr)
+	void mac(int l, int p0, int p1, long slot_blk, cudaStream_t st, double2 *Y = nullptr, const double2 *init = nullptr)
 	{
+		const FirLevel &L = lv[l];
+		const FirLevelPlan &Lp = s.lv[l];
 		MacArgs m = {};
-		m.fdl = L.fdl; m.H = L.H; m.Y = Y ? Y : d_Y; m.init = init; m.N = L.B; m.P = L.R;   // the kernel's P: rows of the ring
-		m.slot0 = (int) (slot_blk % L.R); m.p0 = p0; m.p1 = p1;
-		m.h_ch_stride = (fc == 1) ? 0 : (long) L.P * L.B;
+		m.fdl = L.fdl; m.H = L.H; m.Y = Y ? Y : d_Y; m.init = init; m.N = Lp.B; m.P = Lp.R;   // the kernel's P: rows of the ring
+		m.slot0 = (int) (slot_blk % Lp.R); m.p0 = p0; m.p1 = p1;
+		m.h_ch_stride = (fc == 1) ? 0 : (long) Lp.P * Lp.B;
 		// the last level carries (almost) all the taps: it is the kernel the roofline line is about
-		launch_mac(m, n_sel, fc == 1, (&L == &lv[n_levels - 1]) ? "fir_mac" : "fir_mac_head", st);
+		launch_mac(m, n_sel, fc == 1, (l == s.n_levels - 1) ? "fir_mac" : "fir_mac_head", st);
 	}
 
 	// block `L.blk` of level L is complete in the history ring: X into the FDL, S = MAC, IRFFT.
 	// flags/out as for k_fir_inv.
-	int level_block(FirLevel &L, double *out, long out_ch_stride, int inv_flags, cudaStream_t st)
+	int level_block(int l, double *out, long out_ch_stride, int inv_flags, cudaStream_t st)
 	{
+		FirLevel &L = lv[l];
+		const FirLevelPlan &Lp = s.lv[l];
 		FwdArgs f = {};
-		f.in = d_hist + (L.blk * L.B) % hist_len; f.ch_stride = hist_len; f.valid = L.B;
-		f.spec = L.fdl; f.spec_ch_stride = (long) L.R * L.B; f.slot = (int) (L.blk % L.R); f.tw = L.tw; f.ptw = L.ptw; f.n_ch = n_sel;
-		if (launch_fwd(L.B, f, st)) return -1;
-		mac(L, 0, L.P, L.blk, st);
+		f.in = d_hist + (L.blk * Lp.B) % s.hist_len; f.ch_stride = s.hist_len; f.valid = Lp.B;
+		f.spec = L.fdl; f.spec_ch_stride = (long) Lp.R * Lp.B; f.slot = (int) (L.blk % Lp.R); f.tw = L.tw; f.ptw = L.ptw; f.n_ch = n_sel;
+		if (launch_fwd(Lp.B, f, st)) return -1;
+		mac(l, 0, Lp.P, L.blk, st);
 		InvArgs v = {};
 		v.Y = d_Y; v.out = out; v.out_ch_stride = out_ch_stride; v.carry = L.carry; v.flags = inv_flags; v.tw = L.tw; v.ptw = L.ptw; v.n_ch = n_sel;
-		if (launch_inv(L.B, v, st)) return -1;
+		if (launch_inv(Lp.B, v, st)) return -1;
 		++L.blk;
 		return 0;
 	}
@@ -1936,56 +1681,58 @@ struct FirOp : Op {
 		const bool serial = g_fir_serialize.load(std::memory_order_relaxed) != 0;
 		cudaStream_t us = serial ? st : side, ts = us, bs = serial ? st : side2;
 		bool any = false;
-		for (int l = 1; l < n_levels; ++l) {
+		for (int l = 1; l < s.n_levels; ++l) {
 			FirLevel &L = lv[l];
-			if (abs_pos % L.B != 0) break;   // sizes double: if this one is not complete, none above is
+			const FirLevelPlan &Lp = s.lv[l];
+			if (abs_pos % Lp.B != 0) break;   // sizes double: if this one is not complete, none above is
 			if (!any && us != st) {
 				CUDA_TRY(cudaEventRecord(ev_main, st), return -1);
 				CUDA_TRY(cudaStreamWaitEvent(side, ev_main, 0), return -1);
 			}
 			any = true;
 			L0Args f = {};
-			f.in = d_hist + (L.blk * L.B) % hist_len; f.in_ch_stride = hist_len;
-			f.fdl = L.fdl; f.fdl_ch_stride = (long) L.R * L.B; f.fdl_rows = L.R;
-			f.H = L.H; f.h_ch_stride = (fc == 1) ? 0 : (long) L.P * L.B;
-			f.P = 1; f.slot = (int) (L.blk % L.R);
-			f.out = L.pend; f.out_ch_stride = L.B; f.carry = L.carry; f.tw = L.tw; f.ptw = L.ptw; f.n_ch = n_sel;
-			f.init = (L.tail && L.blk >= 1) ? d_Y_side : nullptr;   // Y of this block: launched one period ago, same stream
-			if (launch_level0(L.B, f, us)) return -1;
+			f.in = d_hist + (L.blk * Lp.B) % s.hist_len; f.in_ch_stride = s.hist_len;
+			f.fdl = L.fdl; f.fdl_ch_stride = (long) Lp.R * Lp.B; f.fdl_rows = Lp.R;
+			f.H = L.H; f.h_ch_stride = (fc == 1) ? 0 : (long) Lp.P * Lp.B;
+			f.P = 1; f.slot = (int) (L.blk % Lp.R);
+			f.out = L.pend; f.out_ch_stride = Lp.B; f.carry = L.carry; f.tw = L.tw; f.ptw = L.ptw; f.n_ch = n_sel;
+			f.init = (Lp.tail && L.blk >= 1) ? d_Y_side : nullptr;   // Y of this block: launched one period ago, same stream
+			if (launch_level0(Lp.B, f, us)) return -1;
 			++L.blk;
 		}
 		if (!any) return 0;
 		CUDA_TRY(cudaEventRecord(ev_urgent, us), return -1);
 		urgent_pending = (us != st);
-		FirLevel &L = lv[n_levels - 1];
-		if (L.tail && tail_pf == 1 && abs_pos % L.B == 0) {
+		const int lt = s.n_levels - 1;
+		const FirLevel &L = lv[lt]; const FirLevelPlan &Lp = s.lv[lt];
+		if (Lp.tail && s.tail_pf == 1 && abs_pos % Lp.B == 0) {
 			const long q1 = L.blk;   // Y_{q+1}, q = the block that just completed
-			if (t_batch > 0) {
+			if (s.t_batch > 0) {
 				// Y_j = U_j + V_j, j = q1: U_j = sum_{1<=p<=T} X_{j-p} H_p now, V_j from the batch launched at
 				// the end of period T*floor((j-2)/T) (zero before the first batch: those blocks do not exist)
-				const int T = t_batch;
+				const int T = s.t_batch;
 				if (q1 >= 2) {
 					const long qb = ((q1 - 2) / T) * T;
 					CUDA_TRY(cudaStreamWaitEvent(ts, ev_batch[(qb / T) & 1], 0), return -1);
 				}
-				const double2 *init = d_V + (size_t) (q1 % (2 * T)) * n_sel * L.B;
-				mac(L, 1, T + 1, q1, ts, d_Y_side, init);
+				const double2 *init = d_V + (size_t) (q1 % (2 * T)) * n_sel * Lp.B;
+				mac(lt, 1, T + 1, q1, ts, d_Y_side, init);
 			}
-			else mac(L, 1, L.P, q1, ts, d_Y_side);
+			else mac(lt, 1, Lp.P, q1, ts, d_Y_side);
 			const long q = q1 - 1;
-			if (t_batch > 0 && q % t_batch == 0) {
+			if (s.t_batch > 0 && q % s.t_batch == 0) {
 				// X_q is in the FDL once the partition-0 kernel of this block has run (ev_urgent on the side stream)
 				CUDA_TRY(cudaStreamWaitEvent(bs, ev_urgent, 0), return -1);
 				MacBatchArgs b = {};
-				b.fdl = L.fdl; b.H = L.H; b.V = d_V; b.N = L.B; b.P = L.P; b.n_sel = n_sel; b.q = q; b.n_slots = 2 * t_batch;
-				b.h_ch_stride = (fc == 1) ? 0 : (long) L.P * L.B;
+				b.fdl = L.fdl; b.H = L.H; b.V = d_V; b.N = Lp.B; b.P = Lp.P; b.n_sel = n_sel; b.q = q; b.n_slots = 2 * s.t_batch;
+				b.h_ch_stride = (fc == 1) ? 0 : (long) Lp.P * Lp.B;
 				b.pf = 1;
-				b.p_lo = t_batch + 1; b.p_hi = L.P;
+				b.p_lo = s.t_batch + 1; b.p_hi = Lp.P;
 				b.g = 0; b.K = 1; b.w = 1;
-				const int threads = (L.B < batch_threads_for(t_batch)) ? L.B : batch_threads_for(t_batch);
-				dim3 grid(L.B / threads, n_sel);
-				launch_mac_batch(t_batch, fc == 1, grid, threads, bs, b);
-				CUDA_TRY(cudaEventRecord(ev_batch[(q / t_batch) & 1], bs), return -1);
+				const int threads = (Lp.B < batch_threads_for(s.t_batch)) ? Lp.B : batch_threads_for(s.t_batch);
+				dim3 grid(Lp.B / threads, n_sel);
+				launch_mac_batch(s.t_batch, fc == 1, grid, threads, bs, b);
+				CUDA_TRY(cudaEventRecord(ev_batch[(q / s.t_batch) & 1], bs), return -1);
 			}
 		}
 		return 0;
@@ -1997,7 +1744,8 @@ struct FirOp : Op {
 	// With time-batching, V_j = sum_{p>=T+2} (T periods per launch, second side stream) is its starting value.
 	int advance_tail0(cudaStream_t st)
 	{
-		FirLevel &L = lv[0];
+		const FirLevel &L = lv[0];
+		const FirLevelPlan &Lp = s.lv[0];
 		const bool serial = g_fir_serialize.load(std::memory_order_relaxed) != 0;
 		// The per-block MAC runs on the side stream, time-slicing with the next fused kernel (a shorter step than with
 		// the MAC queued behind the fused kernel on the caller's stream, where it runs alone -- DSP_B200_FIR_TAIL_MAIN=1
@@ -2006,52 +1754,52 @@ struct FirOp : Op {
 		const bool on_main = serial || tail_main > 0;
 		cudaStream_t ts = on_main ? st : side, bs = serial ? st : side2;
 		const long q = L.blk - 1, j = q + 2;
-		if (use_pipe) {
+		if (s.use_pipe) {
 			// The pipeline kernel of block q does block q's share of the batched tail itself (channels of residue
 			// q % 4: V_{q+2} .. V_{q+5} from the blocks up to q-1).  A block that took the general path gets the same
 			// share from the stand-alone batch kernel, here, on the caller's stream.
-			if (t_batch > 0 && !last_block_piped && q >= 1) {
-				const int g = (int) (q % t_batch);
+			if (s.t_batch > 0 && !last_block_piped && q >= 1) {
+				const int g = (int) (q % s.t_batch);
 				if (n_sel > g) {
 					MacBatchArgs b = {};
-					b.fdl = L.fdl; b.H = L.H; b.V = d_V; b.N = L.B; b.P = L.P; b.n_sel = n_sel; b.q = q - 1; b.n_slots = 2 * t_batch;
-					b.h_ch_stride = (fc == 1) ? 0 : (long) L.P * L.B;
+					b.fdl = L.fdl; b.H = L.H; b.V = d_V; b.N = Lp.B; b.P = Lp.P; b.n_sel = n_sel; b.q = q - 1; b.n_slots = 2 * s.t_batch;
+					b.h_ch_stride = (fc == 1) ? 0 : (long) Lp.P * Lp.B;
 					b.pf = 2;
-					b.p_lo = t_batch + 2; b.p_hi = L.P;
-					b.g = g; b.K = t_batch; b.w = 1;
-					const int threads = (L.B < batch_threads_for(t_batch)) ? L.B : batch_threads_for(t_batch);
-					dim3 grid(L.B / threads, (n_sel - g + t_batch - 1) / t_batch);
-					launch_mac_batch(t_batch, fc == 1, grid, threads, st, b);
+					b.p_lo = s.t_batch + 2; b.p_hi = Lp.P;
+					b.g = g; b.K = s.t_batch; b.w = 1;
+					const int threads = (Lp.B < batch_threads_for(s.t_batch)) ? Lp.B : batch_threads_for(s.t_batch);
+					dim3 grid(Lp.B / threads, (n_sel - g + s.t_batch - 1) / s.t_batch);
+					launch_mac_batch(s.t_batch, fc == 1, grid, threads, st, b);
 				}
 			}
 			return 0;
 		}
-		if (fold) {
+		if (s.fold) {
 			// no per-block MAC: the fused kernel of block j sums the partitions the near tier leaves to it
 			if (!serial) CUDA_TRY(cudaEventRecord(ev_main, st), return -1);
-			if (launch_tiers0(L, q, bs, serial)) return -1;
+			if (launch_tiers0(q, bs, serial)) return -1;
 			ev_bs_at[q & 3] = ev_bs_last;
 			return 0;
 		}
-		double2 *Y = d_Y_side + (size_t) (j & 1) * n_sel * L.B;
+		double2 *Y = d_Y_side + (size_t) (j & 1) * n_sel * Lp.B;
 		if (!serial) {
 			CUDA_TRY(cudaEventRecord(ev_main, st), return -1);
 			if (!on_main) CUDA_TRY(cudaStreamWaitEvent(side, ev_main, 0), return -1);
 		}
-		if (merge_tail) {
+		if (s.merge_tail) {
 			// one grid for the per-block MAC (Y_{q+2}) and this block's class of the batch tier (V_{q+3} .. V_{q+6}); the
 			// MAC starts from V_{q+2}, which the launches up to block q-1 produced (same stream, in order)
 			TailArgs ta = {};
-			ta.m.fdl = L.fdl; ta.m.H = L.H; ta.m.Y = Y; ta.m.init = d_V + (size_t) (j % (2 * t_batch)) * n_sel * L.B;
-			ta.m.N = L.B; ta.m.P = L.R; ta.m.slot0 = (int) (j % L.R); ta.m.p0 = 2; ta.m.p1 = t_batch + 2;
-			ta.m.h_ch_stride = (fc == 1) ? 0 : (long) L.P * L.B;
-			const int g = (int) (q % t_batch);
-			ta.b.fdl = L.fdl; ta.b.H = L.H; ta.b.N = L.B; ta.b.P = L.P; ta.b.n_sel = n_sel; ta.b.q = q;
-			ta.b.V = d_V; ta.b.n_slots = 2 * t_batch; ta.b.h_ch_stride = ta.m.h_ch_stride;
-			ta.b.pf = 2; ta.b.p_lo = t_batch + 2; ta.b.p_hi = L.P;
-			ta.b.g = g; ta.b.K = t_batch; ta.b.w = 1;
-			ta.n_batch_y = (n_sel > g) ? (n_sel - g + t_batch - 1) / t_batch : 0;
-			const dim3 grid(L.B / 256, ta.n_batch_y + n_sel);
+			ta.m.fdl = L.fdl; ta.m.H = L.H; ta.m.Y = Y; ta.m.init = d_V + (size_t) (j % (2 * s.t_batch)) * n_sel * Lp.B;
+			ta.m.N = Lp.B; ta.m.P = Lp.R; ta.m.slot0 = (int) (j % Lp.R); ta.m.p0 = 2; ta.m.p1 = s.t_batch + 2;
+			ta.m.h_ch_stride = (fc == 1) ? 0 : (long) Lp.P * Lp.B;
+			const int g = (int) (q % s.t_batch);
+			ta.b.fdl = L.fdl; ta.b.H = L.H; ta.b.N = Lp.B; ta.b.P = Lp.P; ta.b.n_sel = n_sel; ta.b.q = q;
+			ta.b.V = d_V; ta.b.n_slots = 2 * s.t_batch; ta.b.h_ch_stride = ta.m.h_ch_stride;
+			ta.b.pf = 2; ta.b.p_lo = s.t_batch + 2; ta.b.p_hi = Lp.P;
+			ta.b.g = g; ta.b.K = s.t_batch; ta.b.w = 1;
+			ta.n_batch_y = (n_sel > g) ? (n_sel - g + s.t_batch - 1) / s.t_batch : 0;
+			const dim3 grid(Lp.B / 256, ta.n_batch_y + n_sel);
 			{
 				ProfScope prof("fir_tail", ts);
 				if (fc == 1) LAUNCH((k_fir_tail<4, true>), grid, 256, 0, ts, ta);
@@ -2063,14 +1811,14 @@ struct FirOp : Op {
 			ev_bs_last = e;
 			return 0;
 		}
-		if (t_batch > 0) {
+		if (s.t_batch > 0) {
 			// V_j is complete once every tier launch up to block q-1 is (one stream, in order)
 			if (ev_bs_last) CUDA_TRY(cudaStreamWaitEvent(ts, ev_bs_last, 0), return -1);
-			mac(L, 2, t_batch + 2, j, ts, Y, d_V + (size_t) (j % (2 * t_batch)) * n_sel * L.B);
+			mac(0, 2, s.t_batch + 2, j, ts, Y, d_V + (size_t) (j % (2 * s.t_batch)) * n_sel * Lp.B);
 		}
-		else mac(L, 2, L.P, j, ts, Y);
+		else mac(0, 2, Lp.P, j, ts, Y);
 		CUDA_TRY(cudaEventRecord(ev_tail[j & 1], ts), return -1);
-		if (t_batch > 0 && launch_tiers0(L, q, bs, serial)) return -1;
+		if (s.t_batch > 0 && launch_tiers0(q, bs, serial)) return -1;
 		return 0;
 	}
 
@@ -2082,15 +1830,17 @@ struct FirOp : Op {
 	// channel lies inside one far window of that channel (t_far is a multiple of t_batch, the far launch of the same
 	// block comes first).  Folded, the near tier starts at partition la: period q+la+t gets every partition p >= la+t
 	// (all of them involve blocks up to q only), the fused kernel sums the rest, 0 .. la-1+t.
-	int launch_tiers0(FirLevel &L, long q, cudaStream_t bs, bool serial)
+	int launch_tiers0(long q, cudaStream_t bs, bool serial)
 	{
+		const FirLevel &L = lv[0];
+		const FirLevelPlan &Lp = s.lv[0];
 		bool any = false;
-		for (int i = (t_far > 0) ? 1 : 0; i >= 0; --i) {
-			const int T = i ? t_far : t_batch;
+		for (int i = (s.t_far > 0) ? 1 : 0; i >= 0; --i) {
+			const int T = i ? s.t_far : s.t_batch;
 			// K classes of channel groups take turns, one launch every T / K blocks: K = T when staggered, 1 for whole
 			// launches, far_classes for the far tier in between
-			const int K = stagger ? T : (i ? far_classes : 1);
-			const int w = class_w;
+			const int K = s.stagger ? T : (i ? s.far_classes : 1);
+			const int w = s.class_w;
 			const int period = T / K;
 			if (q % period != 0) continue;
 			auto class_rows = [&](int c) {
@@ -2101,30 +1851,30 @@ struct FirOp : Op {
 			const int g = (int) ((q / period) % K);
 			const int n_y = class_rows(g);
 			// the near tier's grid also holds the mid-window pass of the class whose tier launch came pass_m blocks ago
-			const bool pass = i == 0 && pass_m > 0 && q >= pass_m;
-			const int gp = pass ? (int) ((q - pass_m) % K) : 0;
+			const bool pass = i == 0 && s.pass_m > 0 && q >= s.pass_m;
+			const int gp = pass ? (int) ((q - s.pass_m) % K) : 0;
 			const int n_py = pass ? class_rows(gp) : 0;
 			if (n_y + n_py == 0) continue;
 			if (!any && !serial) CUDA_TRY(cudaStreamWaitEvent(bs, ev_main, 0), return -1);
 			any = true;
 			MacBatchArgs b = {};
-			b.fdl = L.fdl; b.H = L.H; b.N = L.B; b.P = L.P; b.n_sel = n_sel; b.q = q;
+			b.fdl = L.fdl; b.H = L.H; b.N = Lp.B; b.P = Lp.P; b.n_sel = n_sel; b.q = q;
 			b.V = i ? d_V2 : d_V; b.n_slots = 2 * T;
-			b.h_ch_stride = (fc == 1) ? 0 : (long) L.P * L.B;
-			b.pf = i ? 2 + far_e : la - 1;
-			b.p_lo = (i == 0 && fold) ? la : T + b.pf;
-			b.p_hi = (i == 0 && t_far > 0) ? t_far + 2 + far_e : L.P;
-			if (i == 0 && t_far > 0) { b.Vin = d_V2; b.vin_slots = 2 * t_far; }
+			b.h_ch_stride = (fc == 1) ? 0 : (long) Lp.P * Lp.B;
+			b.pf = i ? 2 + s.far_e : s.la - 1;
+			b.p_lo = (i == 0 && s.fold) ? s.la : T + b.pf;
+			b.p_hi = (i == 0 && s.t_far > 0) ? s.t_far + 2 + s.far_e : Lp.P;
+			if (i == 0 && s.t_far > 0) { b.Vin = d_V2; b.vin_slots = 2 * s.t_far; }
 			b.g = g; b.K = K; b.w = w;
-			if (n_py > 0) { b.n_tier_y = n_y; b.pass_g = gp; b.pass_m = pass_m; }
+			if (n_py > 0) { b.n_tier_y = n_y; b.pass_g = gp; b.pass_m = s.pass_m; }
 			int threads = batch_threads_for(T);
 			if ((batch_threads == 128 || batch_threads == 64) && batch_threads < threads) threads = batch_threads;
-			if (L.B < threads) threads = L.B;
-			dim3 grid(L.B / threads, n_y + n_py);
+			if (Lp.B < threads) threads = Lp.B;
+			dim3 grid(Lp.B / threads, n_y + n_py);
 			// whole launches of the far tier: at most one CTA per SM (DSP_B200_FIR_FAR_SMEM_KB, 0 = no cap)
 			static const long far_kb = getenv("DSP_B200_FIR_FAR_SMEM_KB") ? atol(getenv("DSP_B200_FIR_FAR_SMEM_KB")) : 0;
 			launch_mac_batch(T, fc == 1, grid, threads, bs, b, i ? "fir_mac_batch_far" : "fir_mac_batch",
-			                 (i && !stagger && far_kb > 0) ? (size_t) far_kb * 1024 : 0);
+			                 (i && !s.stagger && far_kb > 0) ? (size_t) far_kb * 1024 : 0);
 		}
 		if (any) {
 			cudaEvent_t e = ev_bs[ev_bs_n++ & 7];
@@ -2141,7 +1891,7 @@ struct FirOp : Op {
 	int wait_batch_for(long blk, cudaStream_t st)
 	{
 		(void) blk;
-		if (t_batch > 0 && tail_pf == 2 && !use_pipe && ev_bs_last && !g_fir_serialize.load(std::memory_order_relaxed))
+		if (s.t_batch > 0 && s.tail_pf == 2 && !s.use_pipe && ev_bs_last && !g_fir_serialize.load(std::memory_order_relaxed))
 			CUDA_TRY(cudaStreamWaitEvent(st, ev_bs_last, 0), return -1);
 		return 0;
 	}
@@ -2151,9 +1901,9 @@ struct FirOp : Op {
 	PendArgs pend_args(long first_frame_abs) const
 	{
 		PendArgs p = {};
-		for (int l = 1; l < n_levels; ++l) {
+		for (int l = 1; l < s.n_levels; ++l) {
 			const FirLevel &L = lv[l];
-			p.buf[p.n] = L.pend; p.len[p.n] = L.B; p.off[p.n] = (int) (first_frame_abs % L.B);
+			p.buf[p.n] = L.pend; p.len[p.n] = s.lv[l].B; p.off[p.n] = (int) (first_frame_abs % s.lv[l].B);
 			++p.n;
 		}
 		return p;
@@ -2173,41 +1923,42 @@ struct FirOp : Op {
 	int bulk_blocks(int nb, const double *src, double *d, long dstride, const int *dmap, cudaStream_t st)
 	{
 		FirLevel &L = lv[0];
+		const FirLevelPlan &Lp = s.lv[0];
 		const long C = channels;
-		const long off = (abs_pos % hist_len);
+		const long off = (abs_pos % s.hist_len);
 		// the new frames join the history ring (it holds nb_max blocks; at most one wrap)
 		{
-			const long total = (long) nb * B0, first = (total < hist_len - off) ? total : hist_len - off;
+			const long total = (long) nb * s.B0, first = (total < s.hist_len - off) ? total : s.hist_len - off;
 			dim3 grid(ceil_div(first, 32), ceil_div(n_sel, 32));
-			LAUNCH(k_fir_stash, grid, 256, 0, st, src, C, d_ch_map, d_hist, hist_len, off, (int) first, n_sel);
+			LAUNCH(k_fir_stash, grid, 256, 0, st, src, C, d_ch_map, d_hist, s.hist_len, off, (int) first, n_sel);
 			if (first < total) {
 				dim3 grid2(ceil_div(total - first, 32), ceil_div(n_sel, 32));
-				LAUNCH(k_fir_stash, grid2, 256, 0, st, src + first * C, C, d_ch_map, d_hist, hist_len, 0L, (int) (total - first), n_sel);
+				LAUNCH(k_fir_stash, grid2, 256, 0, st, src + first * C, C, d_ch_map, d_hist, s.hist_len, 0L, (int) (total - first), n_sel);
 			}
 		}
 		FwdArgs f = {};
-		f.in = d_hist; f.ch_stride = hist_len; f.valid = B0;
-		f.spec = L.fdl; f.spec_ch_stride = (long) L.R * B0; f.slot = (int) (L.blk % L.R); f.tw = L.tw; f.ptw = L.ptw; f.n_ch = n_sel;
-		f.ring_len = hist_len; f.ring_off = off; f.slot_rows = L.R;
-		if (launch_fwd(B0, f, st, nb)) return -1;
+		f.in = d_hist; f.ch_stride = s.hist_len; f.valid = s.B0;
+		f.spec = L.fdl; f.spec_ch_stride = (long) Lp.R * s.B0; f.slot = (int) (L.blk % Lp.R); f.tw = L.tw; f.ptw = L.ptw; f.n_ch = n_sel;
+		f.ring_len = s.hist_len; f.ring_off = off; f.slot_rows = Lp.R;
+		if (launch_fwd(s.B0, f, st, nb)) return -1;
 		{
 			MacBulkArgs b = {};
-			b.fdl = L.fdl; b.H = L.H; b.Y = d_Ybulk; b.N = B0; b.P = L.P; b.rows = L.R; b.n_sel = n_sel; b.nb = nb; b.j = L.blk;
-			b.h_ch_stride = (fc == 1) ? 0 : (long) L.P * B0;
-			const int threads = (B0 < 256) ? B0 : 256;
-			dim3 grid(B0 / threads, n_sel);
+			b.fdl = L.fdl; b.H = L.H; b.Y = d_Ybulk; b.N = s.B0; b.P = Lp.P; b.rows = Lp.R; b.n_sel = n_sel; b.nb = nb; b.j = L.blk;
+			b.h_ch_stride = (fc == 1) ? 0 : (long) Lp.P * s.B0;
+			const int threads = (s.B0 < 256) ? s.B0 : 256;
+			dim3 grid(s.B0 / threads, n_sel);
 			ProfScope prof("fir_mac_bulk", st);
 			if (fc == 1) LAUNCH((k_fir_mac_bulk<FIR_NB_MAX, true>), grid, threads, 0, st, b);
 			else LAUNCH((k_fir_mac_bulk<FIR_NB_MAX, false>), grid, threads, 0, st, b);
 		}
 		InvArgs v = {};
-		v.Y = d_Ybulk; v.out = d_lo; v.out_ch_stride = B0; v.carry = d_hi; v.flags = INV_RAW; v.tw = L.tw; v.ptw = L.ptw; v.n_ch = n_sel;
-		if (launch_inv(B0, v, st, nb)) return -1;
+		v.Y = d_Ybulk; v.out = d_lo; v.out_ch_stride = s.B0; v.carry = d_hi; v.flags = INV_RAW; v.tw = L.tw; v.ptw = L.ptw; v.n_ch = n_sel;
+		if (launch_inv(s.B0, v, st, nb)) return -1;
 		{
-			dim3 grid(ceil_div(B0, 32), ceil_div(n_sel, 32), nb);
-			LAUNCH(k_fir_unstash_bulk, grid, 256, 0, st, d_lo, d_hi, L.carry, B0, d, dstride, dmap, n_sel);
+			dim3 grid(ceil_div(s.B0, 32), ceil_div(n_sel, 32), nb);
+			LAUNCH(k_fir_unstash_bulk, grid, 256, 0, st, d_lo, d_hi, L.carry, s.B0, d, dstride, dmap, n_sel);
 		}
-		CUDA_TRY(cudaMemcpyAsync(L.carry, d_hi + (size_t) (nb - 1) * n_sel * B0, (size_t) n_sel * B0 * sizeof(double), cudaMemcpyDeviceToDevice, st), return -1);
+		CUDA_TRY(cudaMemcpyAsync(L.carry, d_hi + (size_t) (nb - 1) * n_sel * s.B0, (size_t) n_sel * s.B0 * sizeof(double), cudaMemcpyDeviceToDevice, st), return -1);
 		L.blk += nb;
 		n_bulk += nb;
 		pre_valid = false;
@@ -2218,10 +1969,10 @@ struct FirOp : Op {
 	{
 		if (pre_valid) return 0;
 		FirLevel &L = lv[0];
-		mac(L, 1, L.P, L.blk, st);   // R: completed level-0 blocks only
+		mac(0, 1, s.lv[0].P, L.blk, st);   // R: completed level-0 blocks only
 		InvArgs v = {};
-		v.Y = d_Y; v.out = d_pre; v.out_ch_stride = B0; v.carry = L.carry; v.flags = INV_OUT; v.tw = L.tw; v.ptw = L.ptw; v.n_ch = n_sel;
-		if (launch_inv(B0, v, st)) return -1;
+		v.Y = d_Y; v.out = d_pre; v.out_ch_stride = s.B0; v.carry = L.carry; v.flags = INV_OUT; v.tw = L.tw; v.ptw = L.ptw; v.n_ch = n_sel;
+		if (launch_inv(s.B0, v, st)) return -1;
 		pre_valid = true;
 		return 0;
 	}
@@ -2241,7 +1992,7 @@ struct FirOp : Op {
 	int keep_for_replay(long frames, const double *in, cudaStream_t st)
 	{
 		if (!replay_open) return 0;
-		if (replay_frames + frames > REPLAY_MAX || replans >= 2 || B0 >= 4096) {
+		if (replay_frames + frames > REPLAY_MAX || replans >= 2 || s.B0 >= 4096) {
 			replay_open = false;
 			dev_free(d_replay);
 			d_replay = nullptr;
@@ -2258,7 +2009,7 @@ struct FirOp : Op {
 
 	int maybe_replan(long frames, cudaStream_t st)
 	{
-		if (!replay_open || !planned || frames < 2L * B0 || replay_frames == 0 && abs_pos > 0) return 0;
+		if (!replay_open || !planned || frames < 2L * s.B0 || replay_frames == 0 && abs_pos > 0) return 0;
 		if (getenv("DSP_B200_FIR_NO_REPLAN")) return 0;
 		const long kept = replay_frames;
 		CUDA_TRY(cudaStreamSynchronize(st), return -1);
@@ -2311,98 +2062,99 @@ struct FirOp : Op {
 		}
 		const long abs0 = abs_pos;
 		FirLevel &L0 = lv[0];
-		const dim3 tgrid_full(ceil_div(B0, 32), ceil_div(n_sel, 32));
+		const FirLevelPlan &Lp0 = s.lv[0];
+		const dim3 tgrid_full(ceil_div(s.B0, 32), ceil_div(n_sel, 32));
 
 		long done = 0;
 		while (done < frames) {
 			const double *src = in + done * C;
 			double *d = dst + done * dstride;
-			if (nb_max > 1 && abs_pos % B0 == 0 && frames - done >= 2L * B0) {
-				long nb = (frames - done) / B0;
-				if (nb > nb_max) nb = nb_max;
+			if (s.nb_max > 1 && abs_pos % s.B0 == 0 && frames - done >= 2L * s.B0) {
+				long nb = (frames - done) / s.B0;
+				if (nb > s.nb_max) nb = s.nb_max;
 				if (bulk_blocks((int) nb, src, d, dstride, dmap, st)) return -1;
-				abs_pos += nb * B0;
-				done += nb * B0;
+				abs_pos += nb * s.B0;
+				done += nb * s.B0;
 				continue;
 			}
-			const int pos = (int) (abs_pos % B0);
-			const long blk_off = (abs_pos - pos) % hist_len;
-			const int seg = (int) ((frames - done < B0 - pos) ? frames - done : B0 - pos);
+			const int pos = (int) (abs_pos % s.B0);
+			const long blk_off = (abs_pos - pos) % s.hist_len;
+			const int seg = (int) ((frames - done < s.B0 - pos) ? frames - done : s.B0 - pos);
 			const PendArgs pend = pend_args(abs_pos);
 			// single-level plans: the fused kernel reads the caller's block and writes the caller's result itself
-			const bool direct = direct_io && n_levels == 1 && pos == 0 && seg == B0 && (L0.P <= 2 || tail_pf == 2);
+			const bool direct = direct_io && s.n_levels == 1 && pos == 0 && seg == s.B0 && (Lp0.P <= 2 || s.tail_pf == 2);
 			// the new frames join the history ring
 			if (!direct) {
 				dim3 grid(ceil_div(seg, 32), ceil_div(n_sel, 32));
-				LAUNCH(k_fir_stash, grid, 256, 0, st, src, C, d_ch_map, d_hist, hist_len, blk_off + pos, seg, n_sel);
+				LAUNCH(k_fir_stash, grid, 256, 0, st, src, C, d_ch_map, d_hist, s.hist_len, blk_off + pos, seg, n_sel);
 			}
-			if (pos == 0 && seg == B0) {
+			if (pos == 0 && seg == s.B0) {
 				// fast path: one whole aligned block
 				last_block_piped = false;
-				if (use_pipe && direct) {
+				if (s.use_pipe && direct) {
 					PipeArgs f = {};
 					f.xin = src; f.xin_stride = C; f.xin_map = d_ch_map;
 					f.yout = d; f.yout_stride = dstride; f.yout_map = dmap;
-					f.fdl = L0.fdl; f.fdl_ch_stride = (long) L0.R * B0; f.fdl_rows = L0.R; f.slot = (int) (L0.blk % L0.R);
-					f.H = L0.H; f.h_ch_stride = (fc == 1) ? 0 : (long) L0.P * B0;
-					f.P = L0.P; f.pf = pipe_pf;
-					f.V = (t_batch > 0) ? d_V : nullptr; f.v_slots = 2 * t_batch; f.blk = L0.blk;
+					f.fdl = L0.fdl; f.fdl_ch_stride = (long) Lp0.R * s.B0; f.fdl_rows = Lp0.R; f.slot = (int) (L0.blk % Lp0.R);
+					f.H = L0.H; f.h_ch_stride = (fc == 1) ? 0 : (long) Lp0.P * s.B0;
+					f.P = Lp0.P; f.pf = s.pipe_pf;
+					f.V = (s.t_batch > 0) ? d_V : nullptr; f.v_slots = 2 * s.t_batch; f.blk = L0.blk;
 					f.carry = L0.carry; f.tw = L0.tw; f.ptw = L0.ptw; f.n_ch = n_sel;
 					f.evict_first = pipe_evict_first;
 					f.fake_io = (pipe_fake_io && C == n_sel && dstride == C) ? 1 : 0;
 					f.no_batch_items = pipe_no_items;
 					f.stats = d_stats;
-					if (launch_pipe(B0, f, st)) return -1;
+					if (launch_pipe(s.B0, f, st)) return -1;
 					++L0.blk;
 					++n_pipe;
 					last_block_piped = true;
 				}
-				else if (use_pipe) {
+				else if (s.use_pipe) {
 					// a whole block that cannot use the direct form (never happens today: direct_io is a plan-time switch)
-					if (level_block(L0, d_ytmp, B0, INV_OUT | INV_UPDATE_CARRY, st)) return -1;
+					if (level_block(0, d_ytmp, s.B0, INV_OUT | INV_UPDATE_CARRY, st)) return -1;
 					++n_general;
 				}
-				else if (L0.P <= 2 || tail_pf == 2) {
+				else if (Lp0.P <= 2 || s.tail_pf == 2) {
 					L0Args f = {};
-					f.in = d_hist + blk_off; f.in_ch_stride = hist_len;
+					f.in = d_hist + blk_off; f.in_ch_stride = s.hist_len;
 					if (direct) {
 						f.xin = src; f.xin_stride = C; f.xin_map = d_ch_map;
 						f.yout = d; f.yout_stride = dstride; f.yout_map = dmap;
 						// four adjacent channels per cluster: needs the selected channels contiguous and 16-byte aligned rows
-						f.cluster_io = cluster_ok && B0 >= 2048 && C % 2 == 0 && dstride % 2 == 0 &&
+						f.cluster_io = cluster_ok && s.B0 >= 2048 && C % 2 == 0 && dstride % 2 == 0 &&
 						               ((reinterpret_cast<size_t>(src) | reinterpret_cast<size_t>(d)) & 15) == 0;
 					}
-					f.fdl = L0.fdl; f.fdl_ch_stride = (long) L0.R * B0; f.fdl_rows = L0.R;
-					f.H = L0.H; f.h_ch_stride = (fc == 1) ? 0 : (long) L0.P * B0;
-					f.P = l0_parts(); f.slot = (int) (L0.blk % L0.R);
-					f.out = d_ytmp; f.out_ch_stride = B0; f.carry = L0.carry; f.tw = L0.tw; f.ptw = L0.ptw; f.n_ch = n_sel;
+					f.fdl = L0.fdl; f.fdl_ch_stride = (long) Lp0.R * s.B0; f.fdl_rows = Lp0.R;
+					f.H = L0.H; f.h_ch_stride = (fc == 1) ? 0 : (long) Lp0.P * s.B0;
+					f.P = s.l0_parts(); f.slot = (int) (L0.blk % Lp0.R);
+					f.out = d_ytmp; f.out_ch_stride = s.B0; f.carry = L0.carry; f.tw = L0.tw; f.ptw = L0.ptw; f.n_ch = n_sel;
 					cudaStream_t ls = st;
 					// (not in a synchronous host call: it works on one block at a time, the two event hops cost it time per
 					// block and the priority buys it nothing; with blocks in flight -- submit/wait -- it pays)
-					const bool use_hot = hot && direct && tail_pf == 2 && !host_mode && !g_fir_serialize.load(std::memory_order_relaxed);
+					const bool use_hot = hot && direct && s.tail_pf == 2 && !host_mode && !g_fir_serialize.load(std::memory_order_relaxed);
 					if (use_hot) {
 						CUDA_TRY(cudaEventRecord(ev_hot_in, st), return -1);
 						CUDA_TRY(cudaStreamWaitEvent(hot, ev_hot_in, 0), return -1);
 						ls = hot;
 					}
-					if (fold) {
+					if (s.fold) {
 						// V_j: complete once the tier launches up to block j-la are, and nothing overwrites its slot before
 						// this kernel is done (see `la`); those launches have read FDL row j % P (blocks up to j-la-1 read
 						// it) as well.  Before block la no launch has covered V_j: it is zero (the blocks it sums do not
 						// exist).
-						if (L0.blk >= la) {
-							if (cudaEvent_t e = ev_bs_at[(L0.blk - la) & 3]) CUDA_TRY(cudaStreamWaitEvent(ls, e, 0), return -1);
-							f.init = d_V + (size_t) (L0.blk % (2 * t_batch)) * n_sel * B0;
+						if (L0.blk >= s.la) {
+							if (cudaEvent_t e = ev_bs_at[(L0.blk - s.la) & 3]) CUDA_TRY(cudaStreamWaitEvent(ls, e, 0), return -1);
+							f.init = d_V + (size_t) (L0.blk % (2 * s.t_batch)) * n_sel * s.B0;
 						}
 						f.blk = L0.blk;
-						f.cls_T = t_batch; f.cls_K = stagger ? t_batch : 1; f.cls_w = class_w; f.la = la; f.pass_m = pass_m;
+						f.cls_T = s.t_batch; f.cls_K = s.stagger ? s.t_batch : 1; f.cls_w = s.class_w; f.la = s.la; f.pass_m = s.pass_m;
 					}
-					else if (tail_pf == 2 && L0.blk >= 2) {
+					else if (s.tail_pf == 2 && L0.blk >= 2) {
 						// Y of this block was launched two blocks ago (advance_tail0)
 						CUDA_TRY(cudaStreamWaitEvent(ls, ev_tail[L0.blk & 1], 0), return -1);
-						f.init = d_Y_side + (size_t) (L0.blk & 1) * n_sel * B0;
+						f.init = d_Y_side + (size_t) (L0.blk & 1) * n_sel * s.B0;
 					}
-					if (launch_level0(B0, f, ls)) return -1;
+					if (launch_level0(s.B0, f, ls)) return -1;
 					if (use_hot) {
 						CUDA_TRY(cudaEventRecord(ev_hot_out, hot), return -1);
 						CUDA_TRY(cudaStreamWaitEvent(st, ev_hot_out, 0), return -1);
@@ -2412,12 +2164,12 @@ struct FirOp : Op {
 					else ++n_fused;
 				}
 				else {
-					if (level_block(L0, d_ytmp, B0, INV_OUT | INV_UPDATE_CARRY, st)) return -1;
+					if (level_block(0, d_ytmp, s.B0, INV_OUT | INV_UPDATE_CARRY, st)) return -1;
 					++n_general;
 				}
 				if (!direct) {
 					side_wait(abs_pos, st);
-					LAUNCH(k_fir_unstash, tgrid_full, 256, 0, st, d_ytmp, (long) B0, pend, d, dstride, dmap, B0, n_sel);
+					LAUNCH(k_fir_unstash, tgrid_full, 256, 0, st, d_ytmp, (long) s.B0, pend, d, dstride, dmap, s.B0, n_sel);
 				}
 				pre_valid = false;
 			}
@@ -2425,21 +2177,21 @@ struct FirOp : Op {
 				if (ensure_pre(st)) return -1;
 				dim3 grid(ceil_div(seg, 128), n_sel);
 				side_wait(abs_pos, st);
-				LAUNCH(k_fir_head, grid, 128, 0, st, d_hist, hist_len, blk_off, d_pre, d_h0, (fc == 1) ? 0L : (long) B0, pend,
-				       d, dstride, dmap, B0, pos, seg);
+				LAUNCH(k_fir_head, grid, 128, 0, st, d_hist, s.hist_len, blk_off, d_pre, d_h0, (fc == 1) ? 0L : (long) s.B0, pend,
+				       d, dstride, dmap, s.B0, pos, seg);
 				++n_head;
-				if (pos + seg == B0) {
+				if (pos + seg == s.B0) {
 					// block complete: X into the FDL, carry = IRFFT(S)[B:2B) (its first half has been emitted already)
 					last_block_piped = false;
 					if (wait_batch_for(L0.blk, st)) return -1;
-					if (level_block(L0, nullptr, 0, INV_UPDATE_CARRY, st)) return -1;
+					if (level_block(0, nullptr, 0, INV_UPDATE_CARRY, st)) return -1;
 					++n_general;
 					pre_valid = false;
 				}
 			}
 			abs_pos += seg;
 			done += seg;
-			if (abs_pos % B0 == 0 && ((tail_pf == 2) ? advance_tail0(st) : advance_upper_levels(st))) return -1;
+			if (abs_pos % s.B0 == 0 && ((s.tail_pf == 2) ? advance_tail0(st) : advance_upper_levels(st))) return -1;
 		}
 
 		if (latency > 0) {

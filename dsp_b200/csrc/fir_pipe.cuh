@@ -27,11 +27,10 @@
 #pragma once
 #include "common.cuh"
 #include "fft.cuh"
+#include "fir_plan.h"
 #include <cstdint>
 
 namespace dspb200 {
-
-constexpr int PIPE_TB = 4;   // batch depth of (b): outputs per pass, = number of channel residues
 
 template <int N>
 struct PipeCfg {

@@ -48,9 +48,9 @@ def folded_bytes_model(plan, h):
 
 
 def plan_from_args(a):
-    """The single-level plan FirOp::plan() makes for 2048..8192-frame blocks at batch depth a.t and look-ahead a.lookahead
-    (3 when absent; the full-wave plan uses 2 with one tier) with the default knobs (no far tier below 48 partitions,
-    the stagger from 16 tail partitions on)."""
+    """The single-level plan fir_schedule() (dsp_b200/csrc/fir_plan.h) makes for 2048..8192-frame blocks at batch depth
+    a.t and look-ahead a.lookahead (3 when absent; the full-wave plan uses 2 with one tier) with the default knobs (no far
+    tier below 48 partitions, the stagger from 16 tail partitions on); tests/test_fir_schedule_cpu.py holds the two equal."""
     P = -(-a.taps // a.block)
     t_far = 8 if P >= 48 and 8 > a.t and 8 % a.t == 0 and P >= 2 * 8 + 2 + a.t else 0
     la = 3 if a.unfolded or t_far else int(getattr(a, "lookahead", None) or 3)

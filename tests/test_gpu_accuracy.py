@@ -6,8 +6,8 @@ multiple of 64 taps -- every partition boundary of every plan), through every pl
 Bound: normalized RMS <= 1e-14, normalized max <= 1e-13 (scale = rms(x) ||h||_2 per channel).  Measured on an
 H100 80GB HBM3 (400 W limit), worst over every FIR case below: RMS 4.8e-16, max 3.3e-15.
 
-FIR plan edges (test_fir_plan_edges_exact and the two tests after it): every boundary FirOp::plan() draws, each case
-asserting its plan and which paths ran, in whole blocks and then ragged calls after reset().  Measured on an H100
+FIR plan edges (test_fir_plan_edges_exact and the two tests after it): every boundary fir_schedule() (fir_plan.h) draws,
+each case asserting its plan and which paths ran, in whole blocks and then ragged calls after reset().  Measured on an H100
 80GB HBM3 (700 W limit), worst normalized RMS / max per group: fused kernel without tail (P = 1, 2) 4.7e-16 /
 2.7e-15; tail, batch and stagger thresholds 4.6e-16 / 2.7e-15; far tier at P = 47 / 48 4.7e-16 / 2.7e-15; batch
 depths 6 and 8 4.2e-16 / 2.7e-15; pipeline kernel with and without batch 4.6e-16 / 2.5e-15; multi-level 4.3e-16 /
@@ -36,8 +36,8 @@ import zlib
 import numpy as np
 import pytest
 
-from accuracy import (H_MAX, RS_RATIOS, RsPacing, biquad_within_ref, dyadic_signal, dyadic_taps, env, exact_conv, fir_nerr,
-                      resample_taps_truth, resample_truth, rs_counts, rs_nerr, taps_norm)
+from accuracy import (F2, F4, FIR_CASES, FIR_EDGES, H_MAX, RS_RATIOS, RsPacing, _fir_plan, _ladder, biquad_within_ref, dyadic_signal,
+                      dyadic_taps, env, exact_conv, fir_nerr, resample_taps_truth, resample_truth, rs_counts, rs_nerr, taps_norm)
 
 pytestmark = pytest.mark.gpu
 FIR_RMS, FIR_MAX = 1e-14, 1e-13
@@ -73,43 +73,6 @@ def ir_family(family, taps, channels, seed=0):
         for c in range(channels):
             h[pos, c] = rng.permutation(vals)[:len(pos)]
     return dyadic_taps(h, H_SHIFT)
-
-
-
-# name: (call frames, taps, channels, block_hint, env, plan check)
-F4, F2 = 4096, 2048
-
-
-def _single(B, P=None):
-    return lambda p: len(p["levels"]) == 1 and p["levels"][0]["B"] == B and (P is None or p["levels"][0]["P"] == P)
-
-
-FIR_CASES = {
-    "multi_64": (64, 20000, 4, 0, {}, lambda p: len(p["levels"]) > 1 and p["levels"][0]["B"] == 64),
-    "multi_300": (300, 50000, 4, 0, {}, lambda p: len(p["levels"]) > 1 and p["levels"][0]["B"] == 256),
-    "multi_1000": (1000, 131072, 4, 0, {}, lambda p: len(p["levels"]) > 1 and p["levels"][0]["B"] == 512),
-    "single_2048_t4": (F2, 131072, 8, F2, dict(DSP_B200_FIR_T=4), lambda p: _single(F2, 64)(p) and p["t_batch"] == 4),
-    "single_2048_t6": (F2, 131072, 8, F2, dict(DSP_B200_FIR_T=6), lambda p: _single(F2, 64)(p) and p["t_batch"] == 6),
-    "single_2048_t8": (F2, 131072, 8, F2, dict(DSP_B200_FIR_T=8), lambda p: _single(F2, 64)(p) and p["t_batch"] == 8),
-    "single_4096_t4": (F4, 131072, 8, F4, dict(DSP_B200_FIR_T=4), lambda p: _single(F4, 32)(p) and p["t_batch"] == 4),
-    "single_4096_t6": (F4, 131072, 8, F4, dict(DSP_B200_FIR_T=6), lambda p: _single(F4, 32)(p) and p["t_batch"] == 6),
-    "single_4096_t8": (F4, 131072, 8, F4, dict(DSP_B200_FIR_T=8), lambda p: _single(F4, 32)(p) and p["t_batch"] == 8),
-    "merge": (F4, 131072, 8, F4, dict(DSP_B200_FIR_MERGE=1), lambda p: _single(F4, 32)(p) and p["merge"] == 1),
-    "pipe_4096": (F4, 131072, 8, F4, dict(DSP_B200_FIR_PIPE=1), lambda p: _single(F4, 32)(p) and p["pipe"] == 1),
-    "pipe_2048": (F2, 70000, 8, F2, dict(DSP_B200_FIR_PIPE=1), lambda p: _single(F2)(p) and p["pipe"] == 1),
-    "bulk_32768": (32768, 50000, 3, 32768, {}, lambda p: p["levels"] == [{"B": 8192, "P": 7}]),
-}
-for _far in (8, 12, 16):
-    for _mode, _e in (("s", dict(DSP_B200_FIR_STAGGER=1)), ("u", dict(DSP_B200_FIR_STAGGER=0)),
-                      ("u2", dict(DSP_B200_FIR_STAGGER=0, DSP_B200_FIR_FAR_CLASSES=2))):
-        if _mode == "u2" and (_far // 2) % 4:
-            continue   # two classes need t_far / 2 to be a multiple of t_batch (4): far tiers 8 and 16
-        _e = dict(_e, DSP_B200_FIR_T2=_far, DSP_B200_FIR_T=4)
-        _cls = 2 if _mode == "u2" else 1
-        FIR_CASES["far%d_%s" % (_far, _mode)] = (
-            F2, 131072, 8, F2, _e,
-            (lambda far, stag, cls: lambda p: _single(F2, 64)(p) and p["t_far"] == far and p["stagger"] == stag
-             and (stag or p["far_classes"] == cls))(_far, 1 if _mode == "s" else 0, _cls))
 
 
 def _run_fir(gpu_lib, x, h, frames, hint, envs, selector=None, latency=0, cuts=None):
@@ -198,104 +161,7 @@ def test_fir_block_io_and_stream_shapes_exact(gpu_lib, case, family):
     assert r <= FIR_RMS and m <= FIR_MAX, (case, family, r, m, plan)
 
 
-# Plan edges: every boundary FirOp::plan() draws, each case with the plan it must make.  A planner change that moves
-# a case off its edge fails the plan assertion instead of quietly testing something else.
-FIR_EDGES = {}
 PATHS = ("fused", "cluster", "pipe", "bulk", "general")   # describe()["paths"]: level-0 blocks per path ("head": launches)
-
-
-def _fir_plan(levels, **kw):
-    """The describe() fields a case must show: levels [(B, P), ...]; tail_pf, t_batch, t_far, stagger, pipe and
-    pipe_pf are 0 and bulk (blocks per bulk launch) is 1 unless given."""
-    p = dict(levels=[{"B": B, "P": P} for B, P in levels], tail_pf=0, t_batch=0, t_far=0, stagger=0, bulk=1, pipe=0, pipe_pf=0)
-    p.update(kw)
-    return p
-
-
-def _edge(group, name, taps, C, hint, plan, envs=None, sel=None, latency=0, rising=False, short=False, lead=(), call=None):
-    """One case: `hint` is the block hint (level 0's B), `call` the frames per call of the whole-block pass (default
-    B0), `lead` the first calls of the ragged pass, `rising` adds the rising family (threshold cases), `short` runs a
-    stream shorter than the filter."""
-    FIR_EDGES["%s/%s" % (group, name)] = dict(taps=taps, C=C, hint=hint, plan=plan, envs=envs or {}, sel=sel, latency=latency,
-                                              rising=rising, short=short, lead=tuple(lead), call=call)
-
-
-def _ladder(B0, last_P, top=4096):
-    """Multi-level plans: level 0 (B0, P = 2), one partition on every level up to `top`, `last_P` on the last."""
-    lv, B = [(B0, 2)], 2 * B0
-    while B < top:
-        lv.append((B, 1))
-        B *= 2
-    return lv + [(top, last_P)]
-
-
-# single level, fused kernel, no tail: P = 1 up to T = B, P = 2 from one tap more
-for _B in (64, F2, F4):
-    for _T, _P in ((1, 1), (2, 1), (_B - 1, 1), (_B, 1), (_B + 1, 2), (2 * _B, 2)):
-        _edge("fused", "B%d_T%d" % (_B, _T), _T, 3 if _B == 64 else 4 if _B == F2 else 5, _B, _fir_plan([(_B, _P)]))
-# single level, tail thresholds: the tail from P = 3, the batch from P = 11, the stagger from P = 22
-for _B in (F2, F4):
-    for _k, _P, _kw, _thr in ((2, 3, {}, False), (10, 10, {}, False), (10, 11, dict(t_batch=4), True),
-                              (21, 21, dict(t_batch=4), False), (21, 22, dict(t_batch=4, stagger=1), True)):
-        _T = _k * _B + (_P - _k)
-        _edge("tail", "B%d_P%d" % (_B, _P), _T, 4 if _B == F2 else 5, _B, _fir_plan([(_B, _P)], tail_pf=2, **_kw), rising=_thr)
-_edge("tail", "B2048_P22_short", 21 * F2 + 1, 4, F2, _fir_plan([(F2, 22)], tail_pf=2, t_batch=4, stagger=1), short=True)
-# far tier from P = 48 (whole launches: no stagger)
-_edge("far", "P47", 47 * F2, 4, F2, _fir_plan([(F2, 47)], tail_pf=2, t_batch=4, stagger=1))
-_edge("far", "P48", 47 * F2 + 1, 4, F2, _fir_plan([(F2, 48)], tail_pf=2, t_batch=4, t_far=8), rising=True)
-# batch depths 6 and 8: the batch from P = 2 T + 3
-for _tb, _k in ((6, 14), (8, 18)):
-    _edge("depth", "T%d_P%d" % (_tb, _k), _k * F2, 4, F2, _fir_plan([(F2, _k)], tail_pf=2), envs=dict(DSP_B200_FIR_T=_tb))
-    _edge("depth", "T%d_P%d" % (_tb, _k + 1), _k * F2 + 1, 4, F2, _fir_plan([(F2, _k + 1)], tail_pf=2, t_batch=_tb),
-          envs=dict(DSP_B200_FIR_T=_tb), rising=True)
-# pipeline kernel: it sums every partition itself (pipe_pf = P) until the batch starts at P = 11
-for _B in (F2, F4):
-    for _T, _P, _kw in ((2 * _B + 1, 3, dict(pipe_pf=3)), (3 * _B + 1, 4, dict(pipe_pf=4)), (10 * _B, 10, dict(pipe_pf=10)),
-                        (10 * _B + 1, 11, dict(pipe_pf=6, t_batch=4))):
-        _edge("pipe", "B%d_P%d" % (_B, _P), _T, 4, _B, _fir_plan([(_B, _P)], tail_pf=2, pipe=1, **_kw),
-              envs=dict(DSP_B200_FIR_PIPE=1), rising=_P == 11)
-# multi-level: an upper level holding one tap, the last level (4096) at P = 1 and 2 (the tail starts), 9 and 10 (the batch)
-for _B0 in (64, 128, 256, 512, 1024):
-    _C = {64: 3, 128: 4, 256: 5, 512: 4, 1024: 2}[_B0]
-    _edge("multi", "B%d_T%d" % (_B0, 2 * _B0 + 1), 2 * _B0 + 1, _C, _B0, _fir_plan([(_B0, 2), (2 * _B0, 1)]))
-    _edge("multi", "B%d_T%d" % (_B0, 4 * _B0), 4 * _B0, _C, _B0, _fir_plan([(_B0, 2), (2 * _B0, 1)]))
-    _edge("multi", "B%d_T%d" % (_B0, 4 * _B0 + 1), 4 * _B0 + 1, _C, _B0, _fir_plan([(_B0, 2), (2 * _B0, 1), (4 * _B0, 1)]))
-    _edge("multi", "B%d_T8192" % _B0, 8192, _C, _B0, _fir_plan(_ladder(_B0, 1)))
-    _edge("multi", "B%d_T8193" % _B0, 8193, _C, _B0, _fir_plan(_ladder(_B0, 2), tail_pf=1), rising=True)
-    _edge("multi", "B%d_T40960" % _B0, 40960, _C, _B0, _fir_plan(_ladder(_B0, 9), tail_pf=1))
-    _edge("multi", "B%d_T40961" % _B0, 40961, _C, _B0, _fir_plan(_ladder(_B0, 10), tail_pf=1, t_batch=4), rising=True)
-_edge("multi", "B256_T40961_short", 40961, 5, 256, _fir_plan(_ladder(256, 10), tail_pf=1, t_batch=4), short=True)
-# the most levels a plan has (FIR_MAX_LEVELS = 8): seven upper levels feed `pend`
-_edge("levels", "B64_cap8192", 131072, 2, 64, _fir_plan(_ladder(64, 15, top=8192), tail_pf=1, t_batch=4),
-      envs=dict(DSP_B200_FIR_LEVEL_CAP=8192), rising=True)
-# bulk form: off at P = 2, from P = 3; calls that bring 2, 3 + 5 frames, 4 and 9 blocks, then 1 and B - 1 frames
-_BULK_LEAD = (1, 8191, 2 * 8192, 3 * 8192 + 5, 4 * 8192, 9 * 8192, 1, 8191)
-for _hint, _nb in ((16384, 2), (32768, 4)):
-    _edge("bulk", "hint%d_P2" % _hint, 16384, 3, _hint, _fir_plan([(8192, 2)]), lead=_BULK_LEAD, call=_hint)
-    _edge("bulk", "hint%d_P3" % _hint, 16385, 3, _hint, _fir_plan([(8192, 3)], bulk=_nb), lead=_BULK_LEAD, call=_hint, rising=True)
-    _edge("bulk", "hint%d_P10" % _hint, 10 * 8192, 3, _hint, _fir_plan([(8192, 10)], bulk=_nb), lead=_BULK_LEAD, call=_hint)
-# FFT tiles: CPB = 256 / (B / 16) channels per CTA; one channel less and one more
-for _B0, _cpb in ((64, 64), (128, 32), (256, 16), (512, 8), (1024, 4)):
-    for _C in (_cpb - 1, _cpb + 1):
-        _edge("cpb", "B%d_C%d" % (_B0, _C), 2 * _B0 + 1, _C, _B0, _fir_plan([(_B0, 2), (2 * _B0, 1)]))
-_edge("cpb", "B2048_C3", F2 + 1, 3, F2, _fir_plan([(F2, 2)]))
-# the fused kernel's cluster form takes 4 contiguous selected channels from an even one: an odd start and a
-# count that is no multiple of 4 fall back to the per-channel form
-for _B in (F2, F4):
-    for _P in (2, 3):
-        _pl = _fir_plan([(_B, _P)], tail_pf=2 if _P == 3 else 0)
-        _T = (_P - 1) * _B + 1
-        _edge("cluster", "B%d_P%d_sel1-4of6" % (_B, _P), _T, 6, _B, _pl, sel=[1 <= c <= 4 for c in range(6)])
-        _edge("cluster", "B%d_P%d_sel2-9of10" % (_B, _P), _T, 10, _B, _pl, sel=[2 <= c <= 9 for c in range(10)])
-        _edge("cluster", "B%d_P%d_all5" % (_B, _P), _T, 5, _B, _pl)
-# fir's latency ring: latencies around the call size, calls shorter and longer than the latency, 1-frame calls
-for _B0 in (64, F4):
-    for _T in (17, 255):
-        _pl = _fir_plan([(64, 1)] if _B0 == 64 and _T == 17 else [(64, 2), (128, 1)] if _B0 == 64 else [(F4, 1)])
-        for _lat in sorted({1, 17, _B0 - 1, _B0, _B0 + 1, 3 * _B0 + 5}):
-            _edge("latency", "B%d_T%d_lat%d" % (_B0, _T, _lat), _T, 3, _B0, _pl, latency=_lat,
-                  lead=(1, 1, max(_lat - 1, 1), _lat, _lat + 1, 1, 2 * _lat + 3, 1, 1, 3 * _lat, 5),
-                  envs=dict(DSP_B200_FIR_NO_REPLAN=1))   # calls longer than 2 B0 keep this plan
 
 
 def _ragged_sizes(rng, N, B, lead=()):
@@ -331,7 +197,7 @@ def _edge_mixes(case):
 
 @pytest.mark.parametrize("case,mix", [(c, m) for c in FIR_EDGES for m in _edge_mixes(c)])
 def test_fir_plan_edges_exact(gpu_lib, case, mix):
-    """Every boundary of FirOp::plan() against the exact convolution, with the plan each case must make asserted
+    """Every boundary of fir_schedule() against the exact convolution, with the plan each case must make asserted
     (describe()), in two passes of one chain: whole aligned blocks, then reset() and ragged calls (_ragged_sizes).
     describe()["paths"] must show which path each pass took.  Streams of at least 2 R + 3 blocks of the last level
     (R: FDL rows), so that every FDL and V-slot ring wraps; the `short` cases stop before the filter's length.  Taps
