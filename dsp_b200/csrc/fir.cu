@@ -23,16 +23,14 @@
 //                       pf = P partitions of S_j from registers, + Y_j (below), inverse transform, overlap.
 //                       On single-level plans it reads the caller's interleaved block and writes the caller's
 //                       result itself (clusters of four adjacent channels share the rows through DSMEM); with a
-//                       batch tier it starts from V_j and sums the partitions the tier left out: 0 .. la-1+t when
-//                       V_j came from the launch after block j-la-t ("folded": no k_fir_mac; the look-ahead la is 3,
-//                       or 2 on the full-wave plan below).
+//                       batch tier it starts from V_j and sums the partitions the tier left out ("folded": no
+//                       k_fir_mac; fir_fused_parts() in fir_plan.h, which holds the whole schedule).
 //   k_fir_mac           Y_j = V_j + sum_{pf<=p<pf+T} X_{j-p} . H_p on a side stream, a block period ahead (the
 //                       blocks it needs were complete pf periods ago): the HBM-streaming kernel
 //   k_fir_mac_batch<T>  V_j = sum_{p>=pf+T} X_{j-p} . H_p for T periods at once (filter rows slide through a
 //                       register window: every FDL and filter row is read once per T outputs); folded, the near
 //                       tier also takes every partition p < pf+T whose block is complete (the triangle p >= la+t);
-//                       on the full-wave plan the same grid runs the mid-window pass of the class launched m blocks
-//                       earlier, which adds partitions la+t-m .. la-1+t to its periods t >= m (FirSchedule::pass_m)
+//                       on the full-wave plan the same grid runs a mid-window pass (FirSchedule::pass_m)
 //   k_fir_mac_bulk<8>   calls that bring several whole 8192-blocks: all partitions of up to 8 new blocks in
 //                       one pass, with one forward and one inverse launch (k_fir_fwd / k_fir_inv, gridDim.y)
 //   k_fir_stash/unstash interleaved <-> per-channel copies for multi-level plans and ragged calls
@@ -284,11 +282,7 @@ struct L0Args {
 	const double2 *H;        // [s or 0][rows][N]
 	long h_ch_stride;
 	int P, slot;             // P: partitions summed (1, 2: compiled in; more: the folded tail, k_fir_level0<N, 0>)
-	// folded tail (cls_T > 0): block blk's V_j of channel s comes from the near-tier launch of its class
-	// c = (s / cls_w) % cls_K that covers j, made la + t blocks earlier, t = (blk - la - c) mod cls_T (la: the look-ahead,
-	// 3 or 2); it holds the partitions from la + t on, the kernel sums 0 .. la - 1 + t (all P = cls_T + la - 1 while no
-	// launch has covered j).  pass_m > 0: the class's mid-window pass after block j-la-t+pass_m has added partitions
-	// la+t-pass_m .. la-1+t for t >= pass_m, the kernel sums 0 .. la-1+t-pass_m there
+	// folded tail (cls_T > 0): block blk sums fir_fused_parts() partitions of channel s
 	long blk;
 	int cls_T, cls_K, cls_w, la, pass_m;
 	double *out;             // [s][out_ch_stride]: first half + carry
@@ -408,8 +402,7 @@ __device__ __forceinline__ double2 cmac(double2 acc, double2 x, double2 h)
 #define FIR_L0_MAXNREG 128
 #endif
 // P: partitions summed, or 0: a run-time count of at most a.P (single-level plans with a batch tier: the "folded" tail,
-// partitions 0 .. la-1+t of a channel whose V_j came from the near-tier launch after block j-la-t, so that no per-block
-// MAC and no Y spectrum round trip are needed)
+// fir_fused_parts(), so that no per-block MAC and no Y spectrum round trip are needed)
 template <int N, int P, bool CL = false>
 __global__ void __launch_bounds__(FftCfg<N>::THREADS) __maxnreg__((N == 4096) ? FIR_L0_MAXNREG : 128) k_fir_level0(L0Args a)
 {
@@ -635,18 +628,8 @@ __global__ void __launch_bounds__(FftCfg<N>::THREADS) __maxnreg__((N == 4096) ? 
 			for (int p = 1; p < P; ++p) mac_partition(p);
 		}
 		else {
-			// (d < 0: the class's first launch covers a later period.  d >= 0 and t >= pass_m: the pass after block
-			// j-la-t+pass_m <= j-la has run too.  The two transform groups of a 2048-point CTA may loop a different
-			// number of times: no barrier inside.)
-			int np = a.P;
-			if (a.cls_T > 0) {
-				const long d = a.blk - a.la - (s >> (__ffs(a.cls_w) - 1)) % a.cls_K;
-				if (d >= 0) {
-					int t = (int) (d % a.cls_T);
-					if (t >= a.pass_m) t -= a.pass_m;
-					np = a.la + t;
-				}
-			}
+			// (the two transform groups of a 2048-point CTA may loop a different number of times: no barrier inside)
+			const int np = (a.cls_T > 0) ? fir_fused_parts(a.blk, s, a.cls_T, a.cls_K, a.cls_w, a.la, a.pass_m, a.P) : a.P;
 #pragma unroll 1
 			for (int p = 1; p < np; ++p) mac_partition(p);
 		}
@@ -863,13 +846,8 @@ __global__ void __launch_bounds__(256, FIR_MAC_MINB) k_fir_mac(MacArgs a)
 // Time-batched tail of the last level.  One launch after block q completes produces V_j for the T periods
 // j = q+pf+1 .. q+pf+T at once (pf = partitions summed inside the fused FFT kernel): every FDL row and every filter
 // row is streamed ONCE for T outputs (the filter rows slide through a T-deep register window), instead of once per
-// output.  V_t[k] = Vin_t[k] + sum_{m>pf} X_{q+pf+1-m}[k] * H_{m+t}[k] over the (m, t) with p_lo <= m+t < p_hi: only
-// blocks up to q.  With p_lo >= pf+T that is V_j = sum_{p in [p_lo, p_hi)} X_{j-p} H_p for every t (the per-block MAC
-// adds the same partitions to every period); with p_lo = pf+1 (the folded near tier) period t gets the partitions
-// p >= pf+1+t -- a triangle of partitions 0 .. pf+T-1 is left to the fused kernel, which sums 0 .. pf+t.
-// Tiers: a deeper batch (larger T) reads the filter less often; the plan stacks two of them -- the far tier's result
-// is the near tier's starting value `Vin`, the near tier's result is what the per-block MAC or the fused kernel starts
-// from.
+// output.  Which partitions a period gets: fir_batch_window() (fir_plan.h).  Tiers: a deeper batch (larger T) reads the
+// filter less often; the far tier's result is the near tier's starting value `Vin`.
 struct MacBatchArgs {
 	const double2 *fdl;   // [s][P][N]
 	const double2 *H;     // [s][P][N] or [P][N]
@@ -878,17 +856,12 @@ struct MacBatchArgs {
 	long q;               // block that just completed
 	int n_slots;
 	long h_ch_stride;
-	int pf;               // partitions 0..pf-1 are summed by the level's fused FFT kernel (1: upper levels, 2: level 0)
-	// channels of this launch: class g of K, the classes taking turns over groups of w adjacent channels; blockIdx.y = y
-	// is channel (g + K (y / w)) w + y % w (0, 1, 1: all channels)
+	// a FirTierLaunch (fir_plan.h): blockIdx.y = y < n_tier_y is row y of class g, the rest the pass rows of class pass_g
+	int pf;
 	int g, K, w;
-	int p_lo, p_hi;       // partitions of this tier
+	int p_lo, p_hi;
 	const double2 *Vin;   // [slot][s][N], slot = j mod vin_slots: a farther tier's sums to start from (NULL: zero)
 	int vin_slots;
-	// the mid-window pass of the folded near tier in the same grid (pass_m > 0): rows y >= n_tier_y are the channels of
-	// class pass_g, whose tier launch after block q - pass_m covered the periods q+pf+1-pass_m .. q+pf+T-pass_m.  Its
-	// periods j = q+pf+1+t, t < T - pass_m, get the partitions p_lo+t .. p_lo+t+pass_m-1 added to V_j in place: pass_m
-	// FDL rows X_q .. X_{q-pass_m+1} and the filter rows p_lo .. p_lo+T-2
 	int n_tier_y, pass_g, pass_m;
 };
 
@@ -907,17 +880,14 @@ struct MacBatchCfg {
 #endif
 };
 
-// PASS: the mid-window pass role (MacBatchArgs::pass_m): the same sliding window with X rows m < x_hi, filter rows
-// p < h_hi and T - pass_m periods, V read and written in place by the thread that owns the element
+// PASS: the mid-window pass role, V read and written in place by the thread that owns the element
 template <int T, bool SHARED_H, bool DCW, bool PASS = false>
 __device__ __forceinline__ void fir_mac_batch_body(const MacBatchArgs &a, int y)
 {
 	const int k = blockIdx.x * blockDim.x + threadIdx.x;
-	const int wl = __ffs(a.w) - 1;   // w: a power of two
-	const int s = (((PASS ? a.pass_g : a.g) + a.K * (y >> wl)) << wl) + (y & (a.w - 1));
-	const int x_hi = PASS ? a.p_lo + a.pass_m : a.p_hi;
-	const int h_hi = PASS ? a.p_lo + T - 1 : a.p_hi;
-	const int n_t = PASS ? T - a.pass_m : T;
+	const int s = fir_class_channel(PASS ? a.pass_g : a.g, a.K, a.w, y);
+	const FirBatchWindow win = fir_batch_window(PASS, T, a.p_lo, a.p_hi, a.pass_m);
+	const int x_hi = win.x_hi, h_hi = win.h_hi, n_t = win.n_t;
 	const double2 *Vin = PASS ? a.V : a.Vin;
 	const int vin_slots = PASS ? a.n_slots : a.vin_slots;
 	const double2 *fdl = a.fdl + (long) s * a.P * a.N + k;
@@ -1706,36 +1676,37 @@ struct FirOp : Op {
 		const int lt = s.n_levels - 1;
 		const FirLevel &L = lv[lt]; const FirLevelPlan &Lp = s.lv[lt];
 		if (Lp.tail && s.tail_pf == 1 && abs_pos % Lp.B == 0) {
-			const long q1 = L.blk;   // Y_{q+1}, q = the block that just completed
-			if (s.t_batch > 0) {
-				// Y_j = U_j + V_j, j = q1: U_j = sum_{1<=p<=T} X_{j-p} H_p now, V_j from the batch launched at
-				// the end of period T*floor((j-2)/T) (zero before the first batch: those blocks do not exist)
-				const int T = s.t_batch;
-				if (q1 >= 2) {
-					const long qb = ((q1 - 2) / T) * T;
-					CUDA_TRY(cudaStreamWaitEvent(ts, ev_batch[(qb / T) & 1], 0), return -1);
-				}
-				const double2 *init = d_V + (size_t) (q1 % (2 * T)) * n_sel * Lp.B;
-				mac(lt, 1, T + 1, q1, ts, d_Y_side, init);
-			}
-			else mac(lt, 1, Lp.P, q1, ts, d_Y_side);
+			const long q1 = L.blk;   // Y_{q+1} = MAC + V_{q+1}, q = the block that just completed
+			const long qb = s.tier_wait(q1);
+			if (qb >= 0) CUDA_TRY(cudaStreamWaitEvent(ts, ev_batch[(qb / s.t_batch) & 1], 0), return -1);
+			const double2 *init = (s.t_batch > 0) ? d_V + (size_t) (q1 % (2 * s.t_batch)) * n_sel * Lp.B : nullptr;
+			mac(lt, s.mac_parts().first, s.mac_parts().second, q1, ts, d_Y_side, init);
 			const long q = q1 - 1;
-			if (s.t_batch > 0 && q % s.t_batch == 0) {
+			const FirTierLaunches tl = fir_tier_launches(s, q, n_sel);
+			if (tl.n > 0) {
 				// X_q is in the FDL once the partition-0 kernel of this block has run (ev_urgent on the side stream)
 				CUDA_TRY(cudaStreamWaitEvent(bs, ev_urgent, 0), return -1);
-				MacBatchArgs b = {};
-				b.fdl = L.fdl; b.H = L.H; b.V = d_V; b.N = Lp.B; b.P = Lp.P; b.n_sel = n_sel; b.q = q; b.n_slots = 2 * s.t_batch;
-				b.h_ch_stride = (fc == 1) ? 0 : (long) Lp.P * Lp.B;
-				b.pf = 1;
-				b.p_lo = s.t_batch + 1; b.p_hi = Lp.P;
-				b.g = 0; b.K = 1; b.w = 1;
 				const int threads = (Lp.B < batch_threads_for(s.t_batch)) ? Lp.B : batch_threads_for(s.t_batch);
-				dim3 grid(Lp.B / threads, n_sel);
-				launch_mac_batch(s.t_batch, fc == 1, grid, threads, bs, b);
+				launch_mac_batch(s.t_batch, fc == 1, dim3(Lp.B / threads, n_sel), threads, bs, batch_args(tl.l[0], q));
 				CUDA_TRY(cudaEventRecord(ev_batch[(q / s.t_batch) & 1], bs), return -1);
 			}
 		}
 		return 0;
+	}
+
+	// the arguments of a tier launch after block q of the tail level
+	MacBatchArgs batch_args(const FirTierLaunch &d, long q) const
+	{
+		const FirLevel &L = lv[s.n_levels - 1];
+		const FirLevelPlan &Lp = s.lv[s.n_levels - 1];
+		MacBatchArgs b = {};
+		b.fdl = L.fdl; b.H = L.H; b.N = Lp.B; b.P = Lp.P; b.n_sel = n_sel; b.q = q;
+		b.V = d.tier ? d_V2 : d_V; b.n_slots = 2 * d.T;
+		b.h_ch_stride = (fc == 1) ? 0 : (long) Lp.P * Lp.B;
+		b.pf = d.pf; b.p_lo = d.p_lo; b.p_hi = d.p_hi; b.g = d.g; b.K = d.K; b.w = d.w;
+		if (d.from_far) { b.Vin = d_V2; b.vin_slots = 2 * s.t_far; }
+		if (d.pass_rows > 0) { b.n_tier_y = d.rows; b.pass_g = d.pass_g; b.pass_m = d.pass_m; }
+		return b;
 	}
 
 	// Single-level plans: after block q of level 0 has entered the FDL (fused kernel or general path), the part
@@ -1759,23 +1730,16 @@ struct FirOp : Op {
 			// q % 4: V_{q+2} .. V_{q+5} from the blocks up to q-1).  A block that took the general path gets the same
 			// share from the stand-alone batch kernel, here, on the caller's stream.
 			if (s.t_batch > 0 && !last_block_piped && q >= 1) {
-				const int g = (int) (q % s.t_batch);
-				if (n_sel > g) {
-					MacBatchArgs b = {};
-					b.fdl = L.fdl; b.H = L.H; b.V = d_V; b.N = Lp.B; b.P = Lp.P; b.n_sel = n_sel; b.q = q - 1; b.n_slots = 2 * s.t_batch;
-					b.h_ch_stride = (fc == 1) ? 0 : (long) Lp.P * Lp.B;
-					b.pf = 2;
-					b.p_lo = s.t_batch + 2; b.p_hi = Lp.P;
-					b.g = g; b.K = s.t_batch; b.w = 1;
-					const int threads = (Lp.B < batch_threads_for(s.t_batch)) ? Lp.B : batch_threads_for(s.t_batch);
-					dim3 grid(Lp.B / threads, (n_sel - g + s.t_batch - 1) / s.t_batch);
-					launch_mac_batch(s.t_batch, fc == 1, grid, threads, st, b);
+				const int T = s.t_batch, g = (int) (q % T), rows = fir_class_rows(n_sel, g, T, 1);
+				if (rows > 0) {
+					const int threads = (Lp.B < batch_threads_for(T)) ? Lp.B : batch_threads_for(T);
+					const FirTierLaunch d = { 0, T, g, T, 1, 2, T + 2, Lp.P, rows, false, 0, 0, 0 };
+					launch_mac_batch(T, fc == 1, dim3(Lp.B / threads, rows), threads, st, batch_args(d, q - 1));
 				}
 			}
 			return 0;
 		}
 		if (s.fold) {
-			// no per-block MAC: the fused kernel of block j sums the partitions the near tier leaves to it
 			if (!serial) CUDA_TRY(cudaEventRecord(ev_main, st), return -1);
 			if (launch_tiers0(q, bs, serial)) return -1;
 			ev_bs_at[q & 3] = ev_bs_last;
@@ -1787,18 +1751,14 @@ struct FirOp : Op {
 			if (!on_main) CUDA_TRY(cudaStreamWaitEvent(side, ev_main, 0), return -1);
 		}
 		if (s.merge_tail) {
-			// one grid for the per-block MAC (Y_{q+2}) and this block's class of the batch tier (V_{q+3} .. V_{q+6}); the
-			// MAC starts from V_{q+2}, which the launches up to block q-1 produced (same stream, in order)
+			// one grid for the per-block MAC (Y_{q+2}) and this block's class of the batch tier
 			TailArgs ta = {};
 			ta.m.fdl = L.fdl; ta.m.H = L.H; ta.m.Y = Y; ta.m.init = d_V + (size_t) (j % (2 * s.t_batch)) * n_sel * Lp.B;
-			ta.m.N = Lp.B; ta.m.P = Lp.R; ta.m.slot0 = (int) (j % Lp.R); ta.m.p0 = 2; ta.m.p1 = s.t_batch + 2;
+			ta.m.N = Lp.B; ta.m.P = Lp.R; ta.m.slot0 = (int) (j % Lp.R); ta.m.p0 = s.mac_parts().first; ta.m.p1 = s.mac_parts().second;
 			ta.m.h_ch_stride = (fc == 1) ? 0 : (long) Lp.P * Lp.B;
-			const int g = (int) (q % s.t_batch);
-			ta.b.fdl = L.fdl; ta.b.H = L.H; ta.b.N = Lp.B; ta.b.P = Lp.P; ta.b.n_sel = n_sel; ta.b.q = q;
-			ta.b.V = d_V; ta.b.n_slots = 2 * s.t_batch; ta.b.h_ch_stride = ta.m.h_ch_stride;
-			ta.b.pf = 2; ta.b.p_lo = s.t_batch + 2; ta.b.p_hi = Lp.P;
-			ta.b.g = g; ta.b.K = s.t_batch; ta.b.w = 1;
-			ta.n_batch_y = (n_sel > g) ? (n_sel - g + s.t_batch - 1) / s.t_batch : 0;
+			const FirTierLaunches tl = fir_tier_launches(s, q, n_sel);
+			ta.b = batch_args(tl.l[0], q);
+			ta.n_batch_y = tl.l[0].rows;
 			const dim3 grid(Lp.B / 256, ta.n_batch_y + n_sel);
 			{
 				ProfScope prof("fir_tail", ts);
@@ -1811,70 +1771,31 @@ struct FirOp : Op {
 			ev_bs_last = e;
 			return 0;
 		}
-		if (s.t_batch > 0) {
-			// V_j is complete once every tier launch up to block q-1 is (one stream, in order)
-			if (ev_bs_last) CUDA_TRY(cudaStreamWaitEvent(ts, ev_bs_last, 0), return -1);
-			mac(0, 2, s.t_batch + 2, j, ts, Y, d_V + (size_t) (j % (2 * s.t_batch)) * n_sel * Lp.B);
-		}
-		else mac(0, 2, Lp.P, j, ts, Y);
+		// the tier launches up to block q-1 = tier_wait(j): every one made so far
+		if (s.t_batch > 0 && ev_bs_last) CUDA_TRY(cudaStreamWaitEvent(ts, ev_bs_last, 0), return -1);
+		mac(0, s.mac_parts().first, s.mac_parts().second, j, ts, Y, (s.t_batch > 0) ? d_V + (size_t) (j % (2 * s.t_batch)) * n_sel * Lp.B : nullptr);
 		CUDA_TRY(cudaEventRecord(ev_tail[j & 1], ts), return -1);
 		if (s.t_batch > 0 && launch_tiers0(q, bs, serial)) return -1;
 		return 0;
 	}
 
-	// Tier launches after block q of a single-level plan (far tier first: the near tier starts from its sums).  A tier
-	// of depth T produces V_j = (farther tier's V_j) + sum_{p in tier} X_{j-p} H_p for the T periods j = q+la ..
-	// q+la-1+T from the blocks up to q (la = 3 unless folded on a full-wave plan; the far tier works far_e periods further
-	// ahead).  Staggered: for the channels s with (s / class_w) mod T == q mod T, every block; otherwise for all channels
-	// when q mod T == 0.  Both ways a channel's periods j are covered exactly once, and the near tier's window of a
-	// channel lies inside one far window of that channel (t_far is a multiple of t_batch, the far launch of the same
-	// block comes first).  Folded, the near tier starts at partition la: period q+la+t gets every partition p >= la+t
-	// (all of them involve blocks up to q only), the fused kernel sums the rest, 0 .. la-1+t.
+	// the tier launches after block q of a single-level plan (fir_tier_launches)
 	int launch_tiers0(long q, cudaStream_t bs, bool serial)
 	{
-		const FirLevel &L = lv[0];
-		const FirLevelPlan &Lp = s.lv[0];
+		const FirTierLaunches tl = fir_tier_launches(s, q, n_sel);
 		bool any = false;
-		for (int i = (s.t_far > 0) ? 1 : 0; i >= 0; --i) {
-			const int T = i ? s.t_far : s.t_batch;
-			// K classes of channel groups take turns, one launch every T / K blocks: K = T when staggered, 1 for whole
-			// launches, far_classes for the far tier in between
-			const int K = s.stagger ? T : (i ? s.far_classes : 1);
-			const int w = s.class_w;
-			const int period = T / K;
-			if (q % period != 0) continue;
-			auto class_rows = [&](int c) {
-				int n = 0;
-				for (int G = c; G * w < n_sel; G += K) n += (n_sel - G * w < w) ? n_sel - G * w : w;
-				return n;
-			};
-			const int g = (int) ((q / period) % K);
-			const int n_y = class_rows(g);
-			// the near tier's grid also holds the mid-window pass of the class whose tier launch came pass_m blocks ago
-			const bool pass = i == 0 && s.pass_m > 0 && q >= s.pass_m;
-			const int gp = pass ? (int) ((q - s.pass_m) % K) : 0;
-			const int n_py = pass ? class_rows(gp) : 0;
-			if (n_y + n_py == 0) continue;
+		for (int i = 0; i < tl.n; ++i) {
+			const FirTierLaunch &d = tl.l[i];
+			if (d.rows + d.pass_rows == 0) continue;
 			if (!any && !serial) CUDA_TRY(cudaStreamWaitEvent(bs, ev_main, 0), return -1);
 			any = true;
-			MacBatchArgs b = {};
-			b.fdl = L.fdl; b.H = L.H; b.N = Lp.B; b.P = Lp.P; b.n_sel = n_sel; b.q = q;
-			b.V = i ? d_V2 : d_V; b.n_slots = 2 * T;
-			b.h_ch_stride = (fc == 1) ? 0 : (long) Lp.P * Lp.B;
-			b.pf = i ? 2 + s.far_e : s.la - 1;
-			b.p_lo = (i == 0 && s.fold) ? s.la : T + b.pf;
-			b.p_hi = (i == 0 && s.t_far > 0) ? s.t_far + 2 + s.far_e : Lp.P;
-			if (i == 0 && s.t_far > 0) { b.Vin = d_V2; b.vin_slots = 2 * s.t_far; }
-			b.g = g; b.K = K; b.w = w;
-			if (n_py > 0) { b.n_tier_y = n_y; b.pass_g = gp; b.pass_m = s.pass_m; }
-			int threads = batch_threads_for(T);
+			int threads = batch_threads_for(d.T);
 			if ((batch_threads == 128 || batch_threads == 64) && batch_threads < threads) threads = batch_threads;
-			if (Lp.B < threads) threads = Lp.B;
-			dim3 grid(Lp.B / threads, n_y + n_py);
+			if (s.B0 < threads) threads = s.B0;
 			// whole launches of the far tier: at most one CTA per SM (DSP_B200_FIR_FAR_SMEM_KB, 0 = no cap)
 			static const long far_kb = getenv("DSP_B200_FIR_FAR_SMEM_KB") ? atol(getenv("DSP_B200_FIR_FAR_SMEM_KB")) : 0;
-			launch_mac_batch(T, fc == 1, grid, threads, bs, b, i ? "fir_mac_batch_far" : "fir_mac_batch",
-			                 (i && !s.stagger && far_kb > 0) ? (size_t) far_kb * 1024 : 0);
+			launch_mac_batch(d.T, fc == 1, dim3(s.B0 / threads, d.rows + d.pass_rows), threads, bs, batch_args(d, q),
+			                 d.tier ? "fir_mac_batch_far" : "fir_mac_batch", (d.tier && !s.stagger && far_kb > 0) ? (size_t) far_kb * 1024 : 0);
 		}
 		if (any) {
 			cudaEvent_t e = ev_bs[ev_bs_n++ & 7];
@@ -1884,10 +1805,8 @@ struct FirOp : Op {
 		return 0;
 	}
 
-	// The main stream may only go on with block `blk` of a single-level tail plan once the tier launches that read FDL
-	// row blk % P (those after the blocks up to blk-la-1) are complete.  The fused kernel's path gets that from waiting
-	// for Y_blk (whose MAC waited for the launches up to blk-3) or, folded, for the launches up to blk-la themselves;
-	// the general path waits here, for all of them.
+	// the general path's block of a single-level tail plan waits for every tier launch made so far (FirSchedule::tier_wait
+	// is what the fused kernel's path waits for)
 	int wait_batch_for(long blk, cudaStream_t st)
 	{
 		(void) blk;
@@ -2138,12 +2057,9 @@ struct FirOp : Op {
 						ls = hot;
 					}
 					if (s.fold) {
-						// V_j: complete once the tier launches up to block j-la are, and nothing overwrites its slot before
-						// this kernel is done (see `la`); those launches have read FDL row j % P (blocks up to j-la-1 read
-						// it) as well.  Before block la no launch has covered V_j: it is zero (the blocks it sums do not
-						// exist).
-						if (L0.blk >= s.la) {
-							if (cudaEvent_t e = ev_bs_at[(L0.blk - s.la) & 3]) CUDA_TRY(cudaStreamWaitEvent(ls, e, 0), return -1);
+						// (before any launch has covered V_j it is zero: the blocks it sums do not exist)
+						if (const long qw = s.tier_wait(L0.blk); qw >= 0) {
+							if (cudaEvent_t e = ev_bs_at[qw & 3]) CUDA_TRY(cudaStreamWaitEvent(ls, e, 0), return -1);
 							f.init = d_V + (size_t) (L0.blk % (2 * s.t_batch)) * n_sel * s.B0;
 						}
 						f.blk = L0.blk;

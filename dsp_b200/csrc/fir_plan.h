@@ -1,10 +1,18 @@
-// fir_plan.h -- K2: the FIR plan policy (which levels, tiers and kernel forms a FirOp uses), host-only: a value chosen
-// from the call's shape and the DSP_B200_FIR_* knobs, tested without a device; fir.cu allocates and launches what it says.
+// fir_plan.h -- K2: the FIR plan policy (which levels, tiers and kernel forms a FirOp uses) and the schedule each plan
+// runs (which launch sums which partitions of which periods, and what it waits for): values chosen from the call's shape
+// and the DSP_B200_FIR_* knobs, tested without a device; fir.cu allocates and launches what they say.
 #pragma once
 #include <cstdio>
 #include <cstdlib>
 #include <optional>
 #include <string>
+#include <utility>
+
+#ifdef __CUDACC__
+#define FIR_HD __host__ __device__ __forceinline__
+#else
+#define FIR_HD inline
+#endif
 
 namespace dspb200 {
 
@@ -88,30 +96,17 @@ struct FirSchedule {
 	// (fir_pipe.cuh), which sums partitions 0 .. pipe_pf-1 (+ the batched V) itself -- no per-block k_fir_mac
 	bool use_pipe = false;
 	int pipe_pf = 0;
-	// folded tail: the fused kernel of block j starts from V_j, which the tier launches up to block j-la complete
+	// folded tail: no per-block MAC; the fused kernel of block j starts from V_j and sums fir_fused_parts() partitions
 	bool fold = false;
 	// look-ahead of the folded near tier: its launch after block q covers the periods q+la .. q+la+T-1, from partition
 	// la + t on for period q+la+t (every block involved is complete).  3 by default; 2 on the full-wave plan (below),
 	// where the fused kernel is the step's critical path and one partition fewer per block shortens it.
-	// Invariants (T = t_batch):
-	//  - the V ring of 2 T slots is safe for T >= la: the next write to V_j's slot is for period j + 2T, by a launch after
-	//    block j + T - la + 1 > j or later, and launches only start once the fused kernel of their block is complete;
-	//  - FDL row j mod P (X_{j-P} until block j overwrites it) is read by the tier launches after blocks up to j-la-1;
-	//    the fused kernel of block j waits for the launches up to j-la, which covers them;
-	//  - the general path (wait_batch_for) still waits for every launch made so far.
 	int la = 3;
 	// mid-window pass (staggered full-wave plans with one tier, la = 2; DSP_B200_FIR_PASS=0|m, default T/2): the grid
 	// launched after block q' also runs a pass for the class whose tier launch came after block q = q' - pass_m.  For
 	// its periods q+la+t with t >= pass_m it adds partitions la+t-pass_m .. la-1+t to V in place (blocks q'-pass_m+1 ..
 	// q'), and the fused kernel sums 0 .. la-1+t-pass_m there: la .. la-1+max(pass_m, T-pass_m) partitions instead of
-	// la .. la-1+T.  Invariants, in addition to those of `la`:
-	//  - the pass after q' reads X_{q'} and waits for the fused kernel of block q', like the tier launch after q';
-	//  - the fused kernel of block j = q+la+t, t >= pass_m, waits for the launches up to j-la = q+t >= q', the pass included;
-	//  - V slots: the pass touches the periods q+la+pass_m .. q+la+T-1; the class's next tier launch (after q+T) writes
-	//    q+T+la .. q+2T+la-1: disjoint in the ring of 2T slots; their next writer, the tier launch after q+2T, comes after
-	//    the fused kernels that read them;
-	//  - FDL: the pass reads only rows newer than the tier launch of the same grid does (q'-pass_m+1 .. q'); the first
-	//    block to overwrite one, q'-pass_m+1+P, waits for the launches up to q'-pass_m+1+P-la >= q' (P >= 2T+3).
+	// la .. la-1+T.
 	int pass_m = 0;
 	// staggered folded plans: the classes take turns over groups of class_w adjacent channels (1 otherwise), so that
 	// the four channels of a cluster sum the same number of partitions and finish together
@@ -127,7 +122,60 @@ struct FirSchedule {
 	int l0_parts_min() const { return fold ? la : l0_parts(); }
 	// at most, once every class has had its mid-window pass (l0_parts() without one)
 	int l0_parts_steady() const { return fold ? la - 1 + ((pass_m > t_batch - pass_m) ? pass_m : t_batch - pass_m) : l0_parts(); }
+	// partitions [first, second) of a tail-level period the per-block MAC sums: from tail_pf up to the near tier's start
+	std::pair<int, int> mac_parts() const { return { tail_pf, (t_batch > 0) ? t_batch + tail_pf : lv[n_levels - 1].P }; }
+	// The consumer of V_j (the fused kernel of block j when folded, else the per-block MAC of period j) is ordered after
+	// the tier launches up to block tier_wait(j) (< 0: none); they run in order on one stream, a launch after block q once
+	// the fused kernel of block q is complete.  T = t_batch.
+	//  - folded: j-la.  V ring of 2T slots, T >= la: the next write to V_j's slot is for period j+2T, after block
+	//    j+T-la+1 > j.  FDL row j mod P (X_{j-P}) is read by the launches up to block j-la-1; the pass after q' reads rows
+	//    q'-pass_m+1 .. q', overwritten by blocks that wait for q'-pass_m+1+P-la >= q'.
+	//  - per-block MAC: j-3, the launches before its own block j-2 (the fused kernel of block j waits for the MAC).
+	//  - merged grid (merge_tail): the grids up to block j-2, one stream.  Upper level: the launch after T floor((j-2)/T).
+	long tier_wait(long j) const
+	{
+		if (t_batch == 0) return -1;
+		if (n_levels > 1) return (j >= 2) ? t_batch * ((j - 2) / t_batch) : -1;
+		return j - (fold ? la : merge_tail ? 2 : 3);
+	}
 };
+
+#ifdef __CUDA_ARCH__
+FIR_HD int fir_log2(int w) { return __ffs(w) - 1; }   // w: a power of two
+#else
+FIR_HD int fir_log2(int w) { return __builtin_ctz(w); }
+#endif
+
+// Channels of a batch-tier launch: K classes take turns over groups of w adjacent channels (w a power of two; 0, 1, 1:
+// all channels).  Row y of class g is channel (g + K (y / w)) w + y % w; class g has fir_class_rows() rows.
+FIR_HD int fir_class_channel(int g, int K, int w, int y) { return ((g + K * (y >> fir_log2(w))) << fir_log2(w)) + (y & (w - 1)); }
+inline int fir_class_rows(int n_sel, int g, int K, int w)
+{
+	int n = 0;
+	for (int G = g; G * w < n_sel; G += K) n += (n_sel - G * w < w) ? n_sel - G * w : w;
+	return n;
+}
+
+// Folded: the fused kernel of block j sums partitions 0 .. n-1 of channel s.  V_j came from its class's near-tier launch
+// after block j-la-t, t = (j - la - class) mod T (partitions from la + t on); for t >= pass_m the pass after block
+// j-la-t+pass_m <= j-la added la+t-pass_m .. la-1+t.  Before the class's first launch (d < 0) V_j is zero: np_max.
+FIR_HD int fir_fused_parts(long blk, int s, int T, int K, int w, int la, int pass_m, int np_max)
+{
+	const long d = blk - la - (s >> fir_log2(w)) % K;
+	if (d < 0) return np_max;
+	int t = (int) (d % T);
+	if (t >= pass_m) t -= pass_m;
+	return la + t;
+}
+
+// The batch kernel's window for a launch after block q: FDL rows m in [pf+1, x_hi) hold X_{q+pf+1-m}; row m meets filter
+// row m+t for period j = q+pf+1+t when p_lo <= m+t < h_hi; periods t < n_t are written.  Tier role: [p_lo, p_hi).  Pass
+// role: blocks q-pass_m+1 .. q, filter rows < p_lo+T-1, the periods the tier launch after q-pass_m covered from t = pass_m.
+struct FirBatchWindow { int x_hi, h_hi, n_t; };
+FIR_HD FirBatchWindow fir_batch_window(bool pass, int T, int p_lo, int p_hi, int pass_m)
+{
+	return pass ? FirBatchWindow{ p_lo + pass_m, p_lo + T - 1, T - pass_m } : FirBatchWindow{ p_hi, p_hi, T };
+}
 
 inline FirSchedule fir_schedule(const FirShape &sh, const FirKnobs &k)
 {
@@ -230,6 +278,42 @@ inline FirSchedule fir_schedule(const FirShape &sh, const FirKnobs &k)
 		while (s.class_w * 2 <= most) s.class_w *= 2;
 	}
 	return s;
+}
+
+// One batch-tier launch after block q of the tail level (k_fir_mac_batch, or the batch rows of k_fir_tail): V_j of the
+// `rows` channels of class g for the periods j = q+pf+1+t (fir_batch_window), started from the far tier's V_j when
+// from_far; pass_rows > 0: the same grid runs the mid-window pass of class pass_g (FirSchedule::pass_m).
+struct FirTierLaunch {
+	int tier;   // 0: near (V), 1: far (V2)
+	int T, g, K, w, pf, p_lo, p_hi, rows;
+	bool from_far;
+	int pass_g, pass_rows, pass_m;
+};
+struct FirTierLaunches { int n = 0; FirTierLaunch l[2]; };
+
+// The tier launches after block q of the tail level, far tier first (the near tier starts from its sums).  Each
+// channel's periods are covered once: staggered, class (s / class_w) mod T every block, else all channels every T-th
+// block (the far tier: far_classes classes in turns); a near window lies inside one far window (t_far is a multiple of
+// t_batch).  Folded, period q+la+t gets every p >= la+t, the fused kernel the rest.  Upper level: all channels every
+// T-th block, pf = 1.  A launch with no rows (fewer channels than classes) is listed but not made.
+inline FirTierLaunches fir_tier_launches(const FirSchedule &s, long q, int n_sel)
+{
+	FirTierLaunches r;
+	const int P = s.lv[s.n_levels - 1].P;
+	if (s.t_batch == 0 || s.use_pipe) return r;
+	for (int i = (s.t_far > 0) ? 1 : 0; i >= 0; --i) {
+		const int T = i ? s.t_far : s.t_batch;
+		const int K = s.stagger ? T : (i ? s.far_classes : 1), w = s.class_w, period = T / K;
+		if (q % period != 0) continue;
+		const int g = (int) ((q / period) % K), rows = fir_class_rows(n_sel, g, K, w);
+		const bool pass = i == 0 && s.pass_m > 0 && q >= s.pass_m;
+		const int gp = pass ? (int) ((q - s.pass_m) % K) : 0, prows = pass ? fir_class_rows(n_sel, gp, K, w) : 0;
+		const int pf = i ? 2 + s.far_e : (s.tail_pf == 1) ? 1 : s.la - 1;
+		const bool from_far = i == 0 && s.t_far > 0;
+		r.l[r.n++] = { i, T, g, K, w, pf, (i == 0 && s.fold) ? s.la : T + pf, from_far ? s.t_far + 2 + s.far_e : P, rows, from_far,
+		               gp, prows, prows > 0 ? s.pass_m : 0 };
+	}
+	return r;
 }
 
 // the schedule's part of FirOp::describe()

@@ -16,7 +16,9 @@ from the reference's own sinc samples; `resample_truth` evaluates the emitted st
 Errors are reported as nerr = rms(got - want) / scale (and nmax with the max): for FIR, scale = rms(x) ||h||_2
 per channel, for resample rms(x) ||G|| per channel (`rs_nerr`), elsewhere scale = rms(want).
 """
+import ctypes
 import os
+import subprocess
 from contextlib import contextmanager
 
 import numpy as np
@@ -303,9 +305,18 @@ def env(**kw):
 
 
 # ------------------------------------------------------------------------------------------------------------
-# FIR plans: the cases tests/test_gpu_accuracy.py runs on the GPU and tests/test_fir_schedule_cpu.py plans on the CPU
+# FIR plans: the cases the GPU tests run and tests/test_fir_schedule_cpu.py and tests/test_fir_tiers_cpu.py plan on the CPU
 # ------------------------------------------------------------------------------------------------------------
 F4, F2 = 4096, 2048
+CSRC = os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file__))), "dsp_b200", "csrc")
+
+
+def header_lib(tmp_dir, name, source):
+    """Compile a C++ driver of the host-only header dsp_b200/csrc/fir_plan.h with g++ alone (no CUDA); -> ctypes.CDLL."""
+    src, so = tmp_dir / (name + ".cpp"), tmp_dir / ("lib%s.so" % name)
+    src.write_text(source)
+    subprocess.run(["g++", "-std=c++17", "-O1", "-Wall", "-Werror", "-shared", "-fPIC", "-I", CSRC, str(src), "-o", str(so)], check=True)
+    return ctypes.CDLL(str(so))
 
 
 def _single(B, P=None):
@@ -438,3 +449,25 @@ for _B0 in (64, F4):
             _edge("latency", "B%d_T%d_lat%d" % (_B0, _T, _lat), _T, 3, _B0, _pl, latency=_lat,
                   lead=(1, 1, max(_lat - 1, 1), _lat, _lat + 1, 1, 2 * _lat + 3, 1, 1, 3 * _lat, 5),
                   envs=dict(DSP_B200_FIR_NO_REPLAN=1))   # calls longer than 2 B0 keep this plan
+
+
+# The folded tail (tests/test_gpu_fir_fold.py), each case run folded and unfolded.  name: (taps, channels, block, envs,
+# plan fields)
+FOLD_CASES = {
+    "headline_B4096_P32": (131072, 8, F4, {}, dict(P=32, t_batch=4, t_far=0, stagger=1)),
+    "B2048_P11": (10 * F2 + 1, 4, F2, {}, dict(P=11, t_batch=4, t_far=0, stagger=0)),
+    "B2048_P22": (21 * F2 + 1, 4, F2, {}, dict(P=22, t_batch=4, t_far=0, stagger=1)),
+    "B2048_P48": (47 * F2 + 1, 4, F2, {}, dict(P=48, t_batch=4, t_far=8, stagger=0)),
+    "B2048_P19_T8": (18 * F2 + 1, 4, F2, dict(DSP_B200_FIR_T=8), dict(P=19, t_batch=8, t_far=0, stagger=0)),
+}
+
+# The mid-window pass (tests/test_gpu_fir_pass.py) at the full-wave channel count, each case also run with
+# DSP_B200_FIR_PASS=0.  name: (taps, block, P, envs, T, m: DSP_B200_FIR_PASS or None for the default T / 2)
+PASS_CASES = {
+    "headline_T8_m2": (131072, F4, 32, {}, 8, 2),
+    "headline_T8_m4": (131072, F4, 32, {}, 8, None),
+    "headline_T8_m6": (131072, F4, 32, {}, 8, 6),
+    "headline_T12_m6": (131072, F4, 32, dict(DSP_B200_FIR_T=12), 12, None),
+    "B2048_P26": (25 * F2 + 1, F2, 26, {}, 8, None),
+    "B2048_P64": (131072, F2, 64, {}, 8, None),
+}

@@ -9,14 +9,12 @@ import ctypes
 import importlib.util
 import json
 import os
-import subprocess
 
 import pytest
 
-from accuracy import F2, F4, FIR_CASES, FIR_EDGES, env
+from accuracy import F2, F4, FIR_CASES, FIR_EDGES, env, header_lib
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-CSRC = os.path.join(ROOT, "dsp_b200", "csrc")
 SMS = 132   # H100 SXM
 
 DRIVER = r"""
@@ -35,11 +33,7 @@ extern "C" int schedule_json(long taps, long hint, int n_sel, int sm_count, char
 
 @pytest.fixture(scope="module")
 def lib(tmp_path_factory):
-    d = tmp_path_factory.mktemp("fir_schedule")
-    src, so = d / "driver.cpp", d / "libfirschedule.so"
-    src.write_text(DRIVER)
-    subprocess.run(["g++", "-std=c++17", "-O1", "-Wall", "-Werror", "-shared", "-fPIC", "-I", CSRC, str(src), "-o", str(so)], check=True)
-    return ctypes.CDLL(str(so))
+    return header_lib(tmp_path_factory.mktemp("fir_schedule"), "firschedule", DRIVER)
 
 
 @pytest.fixture

@@ -11,20 +11,10 @@ import zlib
 import numpy as np
 import pytest
 
-from accuracy import dyadic_signal, env, exact_conv, fir_nerr
-from test_gpu_accuracy import F2, F4, FIR_MAX, FIR_RMS, H_SHIFT, _ragged_sizes, _run_sizes, ir_family
+from accuracy import FOLD_CASES, dyadic_signal, env, exact_conv, fir_nerr
+from test_gpu_accuracy import FIR_MAX, FIR_RMS, H_SHIFT, _ragged_sizes, _run_sizes, ir_family
 
 pytestmark = pytest.mark.gpu
-
-# name: (taps, channels, block, envs, plan fields)
-FOLD_CASES = {
-    "headline_B4096_P32": (131072, 8, F4, {}, dict(P=32, t_batch=4, t_far=0, stagger=1)),
-    "B2048_P11": (10 * F2 + 1, 4, F2, {}, dict(P=11, t_batch=4, t_far=0, stagger=0)),
-    "B2048_P22": (21 * F2 + 1, 4, F2, {}, dict(P=22, t_batch=4, t_far=0, stagger=1)),
-    "B2048_P48": (47 * F2 + 1, 4, F2, {}, dict(P=48, t_batch=4, t_far=8, stagger=0)),
-    "B2048_P19_T8": (18 * F2 + 1, 4, F2, dict(DSP_B200_FIR_T=8), dict(P=19, t_batch=8, t_far=0, stagger=0)),
-}
-
 
 def _run_form(gpu_lib, x, h, B, envs, fold):
     """Whole blocks through run_device, then reset() and ragged calls; -> (whole, ragged, plan, launches, fir_mac

@@ -15,22 +15,12 @@ import zlib
 import numpy as np
 import pytest
 
-from accuracy import dyadic_signal, exact_conv, fir_nerr
+from accuracy import PASS_CASES, dyadic_signal, exact_conv, fir_nerr
 from test_gpu_accuracy import F2, F4, FIR_MAX, FIR_RMS, H_SHIFT, ir_family
 from test_gpu_fir_fold import _run_form
 from test_gpu_fir_full_wave import full_wave_channels
 
 pytestmark = pytest.mark.gpu
-
-# name: (taps, block, P, envs, T, m: DSP_B200_FIR_PASS or None for the default T / 2)
-PASS_CASES = {
-    "headline_T8_m2": (131072, F4, 32, {}, 8, 2),
-    "headline_T8_m4": (131072, F4, 32, {}, 8, None),
-    "headline_T8_m6": (131072, F4, 32, {}, 8, 6),
-    "headline_T12_m6": (131072, F4, 32, dict(DSP_B200_FIR_T=12), 12, None),
-    "B2048_P26": (25 * F2 + 1, F2, 26, {}, 8, None),
-    "B2048_P64": (131072, F2, 64, {}, 8, None),
-}
 
 _inputs = {}
 
