@@ -895,19 +895,26 @@ __device__ __forceinline__ void fir_mac_batch_body(const MacBatchArgs &a, int y)
 	const bool dc = DCW && (k == 0);
 	const double2 zero = make_double2(0.0, 0.0);
 	double2 acc[T], hw[T];
-#define HROW(p) (((p) >= a.p_lo && (p) < h_hi) ? (SHARED_H ? __ldg(&H[(long) (p) * a.N]) : __ldcs(&H[(long) (p) * a.N])) : zero)
+	// A row meets only the filter rows of its window: bit t of `live` says whether hw[t] is one.  The products with the
+	// others are skipped, not multiplied by zero -- an FDL row outside period t's window may hold a NaN or Inf (of a
+	// block this period does not depend on), and 0 x NaN would carry it into V_j.
+#define HLIVE(p) ((p) >= a.p_lo && (p) < h_hi)
+#define HROW(p) (HLIVE(p) ? (SHARED_H ? __ldg(&H[(long) (p) * a.N]) : __ldcs(&H[(long) (p) * a.N])) : zero)
 	int m = a.pf + 1;   // first row: the newest complete block, X_q
+	unsigned live = 0;
 #pragma unroll
 	for (int t = 0; t < T; ++t) {
 		const long j = a.q + a.pf + 1 + t;
 		acc[t] = (Vin && t < n_t) ? __ldcs(&Vin[((j % vin_slots) * a.n_sel + s) * (long) a.N + k]) : zero;
 		hw[t] = HROW(m + t);
+		live |= (unsigned) HLIVE(m + t) << t;
 	}
 	int slot = (int) (a.q % a.P);   // row of X_{q+pf+1-m} = X_q
 #define XROW(d) __ldcs(&fdl[(long) ((slot - (d) < 0) ? slot - (d) + a.P : slot - (d)) * a.N])
-#define STEP(XV, HN)                                                          \
+#define STEP(XV, HN, PN)                                                      \
 	do {                                                                      \
 		_Pragma("unroll") for (int t = 0; t < T; ++t) {                       \
+			if (!((live >> t) & 1u)) continue;                                \
 			if (dc) {                                                         \
 				acc[t].x = fma(XV.x, hw[t].x, acc[t].x);                      \
 				acc[t].y = fma(XV.y, hw[t].y, acc[t].y);                      \
@@ -919,6 +926,7 @@ __device__ __forceinline__ void fir_mac_batch_body(const MacBatchArgs &a, int y)
 		}                                                                     \
 		_Pragma("unroll") for (int t = 0; t + 1 < T; ++t) hw[t] = hw[t + 1];  \
 		hw[T - 1] = HN;                                                       \
+		live = (live >> 1) | ((unsigned) HLIVE(PN) << (T - 1));               \
 	} while (0)
 #if FIR_BATCH_PREFETCH
 	// the eight loads of the NEXT four rows are issued before the current four are used; rows past the tier are zeros
@@ -931,10 +939,10 @@ __device__ __forceinline__ void fir_mac_batch_body(const MacBatchArgs &a, int y)
 		const int mn = m + 4;
 		const double2 nx0 = XROWG(mn, 0), nx1 = XROWG(mn, 1), nx2 = XROWG(mn, 2), nx3 = XROWG(mn, 3);
 		const double2 nh0 = HROW(mn + T), nh1 = HROW(mn + T + 1), nh2 = HROW(mn + T + 2), nh3 = HROW(mn + T + 3);
-		STEP(x0, h0);
-		STEP(x1, h1);
-		STEP(x2, h2);
-		STEP(x3, h3);
+		STEP(x0, h0, m + T);
+		STEP(x1, h1, m + T + 1);
+		STEP(x2, h2, m + T + 2);
+		STEP(x3, h3, m + T + 3);
 		x0 = nx0; x1 = nx1; x2 = nx2; x3 = nx3;
 		h0 = nh0; h1 = nh1; h2 = nh2; h3 = nh3;
 	}
@@ -944,23 +952,24 @@ __device__ __forceinline__ void fir_mac_batch_body(const MacBatchArgs &a, int y)
 		// eight independent 16-byte loads in flight per thread, as in k_fir_mac
 		const double2 x0 = XROW(0), x1 = XROW(1), x2 = XROW(2), x3 = XROW(3);
 		const double2 h0 = HROW(m + T), h1 = HROW(m + T + 1), h2 = HROW(m + T + 2), h3 = HROW(m + T + 3);
-		STEP(x0, h0);
-		STEP(x1, h1);
-		STEP(x2, h2);
-		STEP(x3, h3);
+		STEP(x0, h0, m + T);
+		STEP(x1, h1, m + T + 1);
+		STEP(x2, h2, m + T + 2);
+		STEP(x3, h3, m + T + 3);
 		slot -= 4;
 		if (slot < 0) slot += a.P;
 	}
 	for (; m < x_hi; ++m) {
 		const double2 x0 = XROW(0);
 		const double2 h0 = HROW(m + T);
-		STEP(x0, h0);
+		STEP(x0, h0, m + T);
 		slot = (slot == 0) ? a.P - 1 : slot - 1;
 	}
 #endif
 #undef XROW
 #undef STEP
 #undef HROW
+#undef HLIVE
 #pragma unroll
 	for (int t = 0; t < T; ++t) {
 		const long j = a.q + a.pf + 1 + t;
@@ -1068,19 +1077,26 @@ __global__ void __launch_bounds__(256) k_fir_mac_bulk(MacBulkArgs a)
 	const bool dc = (k == 0);
 	const double2 zero = make_double2(0.0, 0.0);
 	double2 acc[T], hw[T];
-#define HROW(p) (((p) >= 0 && (p) < a.P) ? (SHARED_H ? __ldg(&H[(long) (p) * a.N]) : __ldcs(&H[(long) (p) * a.N])) : zero)
+	// bit i of `live`: hw[i] is a filter row (0 <= d + i < P).  Products with the others are skipped, not multiplied by
+	// zero: the row of a later block of this call (or a stale row past the new ones) may hold a NaN or Inf, and 0 x NaN
+	// would carry it into the outputs of earlier blocks.
+#define HLIVE(p) ((p) >= 0 && (p) < a.P)
+#define HROW(p) (HLIVE(p) ? (SHARED_H ? __ldg(&H[(long) (p) * a.N]) : __ldcs(&H[(long) (p) * a.N])) : zero)
 	// step d = P-1 .. -(T-1): block m = j - d meets H_{d+i} for output i; window hw[i] = H_{d+i}
 	int d = a.P - 1;
+	unsigned live = 0;
 #pragma unroll
 	for (int i = 0; i < T; ++i) {
 		acc[i] = zero;
 		hw[i] = HROW(d + i);
+		live |= (unsigned) HLIVE(d + i) << i;
 	}
 	int slot = (int) (((a.j - d) % a.rows + a.rows) % a.rows);   // row of X_{j-d}; grows by one per step
 #define XROW(e) __ldcs(&fdl[(long) ((slot + (e) >= a.rows) ? slot + (e) - a.rows : slot + (e)) * a.N])
-#define STEP(XV, HN)                                                          \
+#define STEP(XV, HN, PN)                                                      \
 	do {                                                                      \
 		_Pragma("unroll") for (int i = 0; i < T; ++i) {                       \
+			if (!((live >> i) & 1u)) continue;                                \
 			if (dc) {                                                         \
 				acc[i].x = fma(XV.x, hw[i].x, acc[i].x);                      \
 				acc[i].y = fma(XV.y, hw[i].y, acc[i].y);                      \
@@ -1092,16 +1108,17 @@ __global__ void __launch_bounds__(256) k_fir_mac_bulk(MacBulkArgs a)
 		}                                                                     \
 		_Pragma("unroll") for (int i = T - 1; i > 0; --i) hw[i] = hw[i - 1];  \
 		hw[0] = HN;                                                           \
+		live = ((live << 1) | (unsigned) HLIVE(PN)) & ((1u << T) - 1);        \
 	} while (0)
 	const int steps = a.P + T - 1;
 	int n = 0;
 	for (; n + 4 <= steps; n += 4) {
 		const double2 x0 = XROW(0), x1 = XROW(1), x2 = XROW(2), x3 = XROW(3);
 		const double2 h0 = HROW(d - 1), h1 = HROW(d - 2), h2 = HROW(d - 3), h3 = HROW(d - 4);
-		STEP(x0, h0);
-		STEP(x1, h1);
-		STEP(x2, h2);
-		STEP(x3, h3);
+		STEP(x0, h0, d - 1);
+		STEP(x1, h1, d - 2);
+		STEP(x2, h2, d - 3);
+		STEP(x3, h3, d - 4);
 		d -= 4;
 		slot += 4;
 		if (slot >= a.rows) slot -= a.rows;
@@ -1109,13 +1126,14 @@ __global__ void __launch_bounds__(256) k_fir_mac_bulk(MacBulkArgs a)
 	for (; n < steps; ++n) {
 		const double2 x0 = XROW(0);
 		const double2 h0 = HROW(d - 1);
-		STEP(x0, h0);
+		STEP(x0, h0, d - 1);
 		d -= 1;
 		slot = (slot + 1 == a.rows) ? 0 : slot + 1;
 	}
 #undef XROW
 #undef STEP
 #undef HROW
+#undef HLIVE
 #pragma unroll
 	for (int i = 0; i < T; ++i)
 		if (i < a.nb) a.Y[((long) i * a.n_sel + s) * a.N + k] = acc[i];

@@ -339,6 +339,9 @@ __global__ void __maxnreg__(FIR_PIPE_MAXNREG) k_fir_pipe(PipeArgs a)
 		unsigned phase = 0;
 		const double2 zero = make_double2(0.0, 0.0);
 		double2 accS[PER], accB[TB][PER], hw[TB][PER];
+		// bit u: hw[u] is a filter row of the batch window; products with the zero rows around it are skipped, so that a
+		// NaN or Inf in an FDL row outside a period's window stays out of that period's V (0 x NaN = NaN)
+		unsigned liveB = 0;
 #pragma unroll
 		for (int i = 0; i < PER; ++i) {
 			accS[i] = zero;
@@ -368,18 +371,21 @@ __global__ void __maxnreg__(FIR_PIPE_MAXNREG) k_fir_pipe(PipeArgs a)
 					if (dc && i == 0) {
 #pragma unroll
 						for (int u = 0; u < TB; ++u) {
+							if (!((liveB >> u) & 1u)) continue;
 							accB[u][i].x = fma(x.x, hw[u][i].x, accB[u][i].x);
 							accB[u][i].y = fma(x.y, hw[u][i].y, accB[u][i].y);
 						}
 					}
 					else {
 #pragma unroll
-						for (int u = 0; u < TB; ++u) accB[u][i] = pipe_cmac(accB[u][i], x, hw[u][i]);
+						for (int u = 0; u < TB; ++u)
+							if ((liveB >> u) & 1u) accB[u][i] = pipe_cmac(accB[u][i], x, hw[u][i]);
 					}
 #pragma unroll
 					for (int u = 0; u + 1 < TB; ++u) hw[u][i] = hw[u + 1][i];
 					hw[TB - 1][i] = hn;
 				}
+				liveB = (liveB >> 1) | ((fl & PC_BHASH) ? 1u << (TB - 1) : 0u);
 				if (fl & PC_BSTORE) {
 #pragma unroll
 					for (int u = 0; u < TB; ++u) {
@@ -432,6 +438,7 @@ __global__ void __maxnreg__(FIR_PIPE_MAXNREG) k_fir_pipe(PipeArgs a)
 					for (int u = 0; u < TB; ++u) { accB[u][i] = zero; hw[u][i] = zero; }
 					if (fl & PC_BHASH) hw[TB - 1][i] = Hs[tm + i * TM];
 				}
+				liveB = (fl & PC_BHASH) ? 1u << (TB - 1) : 0u;
 			}
 			}
 			__syncwarp();

@@ -471,3 +471,72 @@ PASS_CASES = {
     "B2048_P26": (25 * F2 + 1, F2, 26, {}, 8, None),
     "B2048_P64": (131072, F2, 64, {}, 8, None),
 }
+
+
+# ------------------------------------------------------------------------------------------------------------
+# Non-finite samples (tests/test_gpu_nonfinite.py): which output frames may depend on one input frame n
+# ------------------------------------------------------------------------------------------------------------
+def fir_b0(hint):
+    """Level 0's B for calls (or a block hint) of `hint` frames: fir_schedule() (fir_plan.h)."""
+    B = 64
+    while 2 * B <= hint and B < 8192:
+        B *= 2
+    return B
+
+
+def fir_level_taps(levels, taps):
+    """[(B, tap0, tap1)] per level of a describe() plan: level 0 from tap 0, level l > 0 from tap B_l, every level
+    P_l partitions of B_l taps, the last one ending at the filter's end (fir_schedule())."""
+    out = []
+    for i, L in enumerate(levels):
+        t0 = 0 if i == 0 else L["B"]
+        out.append((L["B"], t0, min(taps, t0 + L["P"] * L["B"])))
+    return out
+
+
+def fir_nan_window(n, taps, levels, latency=0):
+    """[first, end): the output frames of one FIR channel that may differ when its input frame n changes.
+    A level of block B sums, for output block m (frames m B .. m B + B - 1, before the latency), X_{m - tap0/B - p} H_p
+    over its partitions p < P, where X_j is the 2B-point transform of input blocks j - 1 and j.  An FFT spreads a
+    non-finite input over every bin, so X_k and X_{k+1} (k = n // B) are wholly non-finite, and so is every output block
+    they reach:
+      - first: level 0 (tap0 = 0) reaches output block n // B0 from its start; an upper level starts at tap0 = B
+        and reaches block k + 2 at the earliest, after n.  So first = B0 floor(n / B0) + latency, and nothing earlier
+        may differ (the head kernel of a ragged call, a time-domain product, is later than that too).
+      - end: the last level (B = B_last, P partitions from tap0) reaches up to output block k + 1 + tap0/B + P - 1,
+        which ends at (k + 1) B + tap0 + P B <= (k + 2) B + taps - 1 <= n + 2 B + taps - 1; lower levels end earlier.
+        So end = n + taps + 2 B_last + latency, with a margin of (n mod B_last) + (tap0 + P B_last - taps) + 1.
+    Every tier, look-ahead and pass of the schedule (fir_plan.h) only re-associates those sums, so stale state that
+    the schedule reads with a zero weight is what would break these bounds."""
+    B0, Bl = levels[0]["B"], levels[-1]["B"]
+    return n // B0 * B0 + latency, n + taps + 2 * Bl + latency
+
+
+# Output frames per CTA of each resampler variant (DSP_B200_RS_TILE): RsCfg<R, CH, WARPS>::Q = R WARPS of the FMA
+# kernel's instantiations (tile 1: 16 x 4 warps, 2: 16 x 2, 3: 8 x 4) and RSM_Q of the tensor-core kernels (resample.cu).
+RS_TILE_Q = {1: 64, 2: 32, 3: 32, 4: 32, 5: 32, 6: 32, 7: 32}
+
+
+def rs_nan_windows(n, counts, n_, d, in_len, out_delay, Q):
+    """(exact, tile): boolean masks over the emitted outputs (calls of `counts` frames, drain polls included) of which
+    outputs read input frame n.  exact: n in the output's own window floor(m d / n_) - in_len + 1 .. floor(m d / n_),
+    m = out_delay + q (resample.cu header).  tile: n in the rows the output's CTA tile reads.  A launch covers one
+    call's outputs in tiles of Q, the first at the call's first output; each tile walks the input rows down from the
+    window end of its last output, i_top, to the window start of its first, i_bot (not below row 0), in steps of 4 rows
+    (k_rs_poly's RS_G-row stages, the DMMA's k = 4), and multiplies every row with every output's tap -- zero where
+    the row is outside that output's window (G's rows are zero-padded) or past i_bot.  0 x NaN = NaN, so a non-finite
+    input reaches every output of the tiles that read it: up to Q - 1 outputs before its exact window, and outputs
+    up to 3 rows past it."""
+    q = np.arange(int(np.sum(counts)), dtype=np.int64)
+    ih = (out_delay + q) * d // n_
+    exact = (ih - in_len + 1 <= n) & (n <= ih)
+    tile = np.zeros(q.size, dtype=bool)
+    pos = 0
+    for k in counts:
+        for a in range(pos, pos + k, Q):
+            b = min(a + Q, pos + k) - 1
+            top, bot = ih[b], max(ih[a] - in_len + 1, 0)
+            if top - 4 * -(-(top - bot + 1) // 4) + 1 <= n <= top:
+                tile[a:b + 1] = True
+        pos += k
+    return exact, tile
