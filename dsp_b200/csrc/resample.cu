@@ -177,9 +177,25 @@ __device__ __forceinline__ void rs_load_rows(double (&x)[RS_G][CH], const double
 	}
 }
 
+// Stores of 2 or 4 adjacent output channels.  `out16` (uniform: the caller's `out` is 16-byte aligned, and every
+// store address is `out` plus a multiple of 16 bytes) picks 128-bit stores; without it the same values go out as
+// 64-bit stores, so that an `out` that is only 8-byte aligned (legal for double) takes the same bits.
+__device__ __forceinline__ void rs_store2(double *o, bool out16, double a, double b)
+{
+	if (out16) *reinterpret_cast<double2 *>(o) = make_double2(a, b);
+	else { o[0] = a; o[1] = b; }
+}
+
+__device__ __forceinline__ void rs_store4(double *o, bool out16, double a, double b, double c, double d)
+{
+	rs_store2(o, out16, a, b);
+	rs_store2(o + 2, out16, c, d);
+}
+
 template <int R, int CH, int WARPS, int MINB>
 __global__ void __launch_bounds__(32 * WARPS, MINB) k_rs_poly(const double *__restrict__ ring, long ring_len, int C, const double *__restrict__ G,
-                                                              int g_stride, int pad, int n, int d, int in_len, long m0, long n_out, double *__restrict__ out)
+                                                              int g_stride, int pad, int n, int d, int in_len, long m0, long n_out, double *__restrict__ out,
+                                                              bool out16)
 {
 	using Cfg = RsCfg<R, CH, WARPS>;
 	constexpr int Q = Cfg::Q, LD = Cfg::LD, ROWS = Cfg::ROWS;
@@ -247,11 +263,8 @@ __global__ void __launch_bounds__(32 * WARPS, MINB) k_rs_poly(const double *__re
 		const long q = q0 + warp * R + r;
 		if (q >= n_out) break;
 		double *o = out + q * C + c0;
-		if (CH == 4) {
-			*reinterpret_cast<double2 *>(o) = make_double2(acc[r][0], acc[r][1 % CH]);
-			*reinterpret_cast<double2 *>(o + 2) = make_double2(acc[r][2 % CH], acc[r][3 % CH]);
-		}
-		else if (CH == 2) *reinterpret_cast<double2 *>(o) = make_double2(acc[r][0], acc[r][1 % CH]);
+		if (CH == 4) rs_store4(o, out16, acc[r][0], acc[r][1 % CH], acc[r][2 % CH], acc[r][3 % CH]);
+		else if (CH == 2) rs_store2(o, out16, acc[r][0], acc[r][1 % CH]);
 		else o[0] = acc[r][0];
 	}
 }
@@ -280,7 +293,8 @@ constexpr int RSM_Q = 32, RSM_LD = 40, RSM_ROWS = 128;
 
 template <int WARPS>
 __global__ void __launch_bounds__(32 * WARPS, (WARPS == 4) ? 4 : 1) k_rs_mma(const double *__restrict__ ring, long ring_len, int C, const double *__restrict__ G,
-                                                       int g_stride, int pad, int n, int d, int in_len, long m0, long n_out, double *__restrict__ out)
+                                                       int g_stride, int pad, int n, int d, int in_len, long m0, long n_out, double *__restrict__ out,
+                                                       bool out16)
 {
 	constexpr int MT = 4, NT = 4, Q = RSM_Q, LD = RSM_LD, ROWS = RSM_ROWS;
 	__shared__ __align__(16) double S[ROWS * LD];
@@ -361,14 +375,8 @@ __global__ void __launch_bounds__(32 * WARPS, (WARPS == 4) ? 4 : 1) k_rs_mma(con
 		const long q = q0 + 8 * mt + g;
 		if (q >= n_out) continue;
 		double *o = out + q * C + ch;
-		if (ch < C) {
-			*reinterpret_cast<double2 *>(o) = make_double2(acc[mt][0][0], acc[mt][1][0]);
-			*reinterpret_cast<double2 *>(o + 2) = make_double2(acc[mt][2][0], acc[mt][3][0]);
-		}
-		if (ch + 4 < C) {
-			*reinterpret_cast<double2 *>(o + 4) = make_double2(acc[mt][0][1], acc[mt][1][1]);
-			*reinterpret_cast<double2 *>(o + 6) = make_double2(acc[mt][2][1], acc[mt][3][1]);
-		}
+		if (ch < C) rs_store4(o, out16, acc[mt][0][0], acc[mt][1][0], acc[mt][2][0], acc[mt][3][0]);
+		if (ch + 4 < C) rs_store4(o + 4, out16, acc[mt][0][1], acc[mt][1][1], acc[mt][2][1], acc[mt][3][1]);
 	}
 }
 
@@ -390,7 +398,8 @@ __device__ __forceinline__ void cp_async8(double *smem_dst, const double *gsrc, 
 // single-buffered form spends much of its time waiting for them)
 template <int WARPS, int MINB, int DEPTH>
 __global__ void __launch_bounds__(32 * WARPS, MINB) k_rs_mma2(const double *__restrict__ ring, long ring_len, int C, const double *__restrict__ G,
-                                                        int g_stride, int pad, int n, int d, int in_len, long m0, long n_out, double *__restrict__ out)
+                                                        int g_stride, int pad, int n, int d, int in_len, long m0, long n_out, double *__restrict__ out,
+                                                        bool out16)
 {
 	constexpr int MT = 4, NT = 4, Q = RSM_Q, LD = RSM_LD, ROWS = RSM2_ROWS;
 	__shared__ __align__(16) double S[2][ROWS * LD];
@@ -484,24 +493,18 @@ __global__ void __launch_bounds__(32 * WARPS, MINB) k_rs_mma2(const double *__re
 		const long q = q0 + 8 * mt + g;
 		if (q >= n_out) continue;
 		double *o = out + q * C + ch;
-		if (ch < C) {
-			*reinterpret_cast<double2 *>(o) = make_double2(acc[mt][0][0], acc[mt][1][0]);
-			*reinterpret_cast<double2 *>(o + 2) = make_double2(acc[mt][2][0], acc[mt][3][0]);
-		}
-		if (ch + 4 < C) {
-			*reinterpret_cast<double2 *>(o + 4) = make_double2(acc[mt][0][1], acc[mt][1][1]);
-			*reinterpret_cast<double2 *>(o + 6) = make_double2(acc[mt][2][1], acc[mt][3][1]);
-		}
+		if (ch < C) rs_store4(o, out16, acc[mt][0][0], acc[mt][1][0], acc[mt][2][0], acc[mt][3][0]);
+		if (ch + 4 < C) rs_store4(o + 4, out16, acc[mt][0][1], acc[mt][1][1], acc[mt][2][1], acc[mt][3][1]);
 	}
 }
 
 template <int R, int CH, int WARPS, int MINB>
 static void rs_launch(cudaStream_t st, const double *ring, long ring_len, int C, const double *G, int g_stride, int pad,
-                      const ResampleParams &p, long m0, long n_out, double *out)
+                      const ResampleParams &p, long m0, long n_out, double *out, bool out16)
 {
 	using Cfg = RsCfg<R, CH, WARPS>;
 	const dim3 grid((unsigned) ceil_div(n_out, Cfg::Q), (unsigned) ceil_div(C, 32 * CH));
-	LAUNCH((k_rs_poly<R, CH, WARPS, MINB>), grid, Cfg::THREADS, 0, st, ring, ring_len, C, G, g_stride, pad, p.n, p.d, p.in_len, m0, n_out, out);
+	LAUNCH((k_rs_poly<R, CH, WARPS, MINB>), grid, Cfg::THREADS, 0, st, ring, ring_len, C, G, g_stride, pad, p.n, p.d, p.in_len, m0, n_out, out, out16);
 }
 
 // move the live rows of the input ring into a bigger ring (absolute frame a lives at a % len)
@@ -529,9 +532,10 @@ struct ResampleOp : Op {
 	// kernel, 5..7 the same with the tap tile double-buffered (cp.async) and the input rows requested 2 / 3 / 2 steps
 	// ahead at 4 / 3 / 3 CTAs per SM.  A forced tile the channel count cannot use falls back to the default.
 	int force_tile = 0;
-	// the last launch, for describe(): kernel, tile, warps per CTA, input-row steps requested ahead (0: FMA kernel)
+	// the last launch, for describe(): kernel, tile, warps per CTA, input-row steps requested ahead (0: FMA kernel),
+	// alignment of the output in bytes (16: 128-bit stores, 8: 64-bit stores)
 	const char *last_kernel = "";
-	int last_tile = 0, last_warps = 0, last_depth = 0;
+	int last_tile = 0, last_warps = 0, last_depth = 0, last_out_align = 0;
 
 	const char *name() const override { return "resample"; }
 
@@ -539,8 +543,8 @@ struct ResampleOp : Op {
 	{
 		char buf[384];
 		snprintf(buf, sizeof(buf), "{\"op\":\"resample\",\"n\":%d,\"d\":%d,\"in_len\":%d,\"out_len\":%d,\"out_delay\":%d,\"ring_len\":%ld,"
-		         "\"force_tile\":%d,\"kernel\":\"%s\",\"tile\":%d,\"warps\":%d,\"depth\":%d}",
-		         p.n, p.d, p.in_len, p.out_len, p.out_delay, ring_len, force_tile, last_kernel, last_tile, last_warps, last_depth);
+		         "\"force_tile\":%d,\"kernel\":\"%s\",\"tile\":%d,\"warps\":%d,\"depth\":%d,\"out_align\":%d}",
+		         p.n, p.d, p.in_len, p.out_len, p.out_delay, ring_len, force_tile, last_kernel, last_tile, last_warps, last_depth, last_out_align);
 		return buf;
 	}
 	~ResampleOp() override { dev_free(d_G); dev_free(d_ring); }
@@ -630,11 +634,15 @@ struct ResampleOp : Op {
 			const long sms = sm_count();   // the tensor-core kernels: warps per CTA as long as every SM still gets a few CTAs
 			if (sms < 1) return -1;
 			last_tile = tile;
+			// the stores into the caller's rows: 128-bit when `out` allows it (a row offset is a multiple of 16 bytes
+			// wherever a kernel stores pairs), else 64-bit -- the same values either way
+			const bool out16 = (reinterpret_cast<uintptr_t>(out) & 15) == 0;
+			last_out_align = out16 ? 16 : 8;
 			if (tile >= 5) {
 				const long tiles = ceil_div(oframes, RSM_Q);
 				const int w = (C >= 128 && tiles * ceil_div(C, 128) >= sms * 3) ? 4 : (C >= 64 && tiles * ceil_div(C, 64) >= sms * 2) ? 2 : 1;
 				const dim3 grid((unsigned) tiles, (unsigned) ceil_div(C, 32 * w));
-#define RS_MMA2(W, MINB, DEPTH) LAUNCH((k_rs_mma2<W, MINB, DEPTH>), grid, 32 * W, 0, st, d_ring, ring_len, C, d_G, g_stride, g_pad, p.n, p.d, p.in_len, first_m, oframes, out)
+#define RS_MMA2(W, MINB, DEPTH) LAUNCH((k_rs_mma2<W, MINB, DEPTH>), grid, 32 * W, 0, st, d_ring, ring_len, C, d_G, g_stride, g_pad, p.n, p.d, p.in_len, first_m, oframes, out, out16)
 				if (w == 4 && tile == 5) RS_MMA2(4, 4, 2);
 				else if (w == 4 && tile == 6) RS_MMA2(4, 3, 3);
 				else if (w == 4) RS_MMA2(4, 3, 2);
@@ -650,17 +658,17 @@ struct ResampleOp : Op {
 				const long tiles = ceil_div(oframes, RSM_Q);
 				const int w = (C >= 128 && tiles * ceil_div(C, 128) >= sms * 3) ? 4 : (C >= 64 && tiles * ceil_div(C, 64) >= sms * 2) ? 2 : 1;
 				const dim3 grid((unsigned) tiles, (unsigned) ceil_div(C, 32 * w));
-				if (w == 4) LAUNCH((k_rs_mma<4>), grid, 128, 0, st, d_ring, ring_len, C, d_G, g_stride, g_pad, p.n, p.d, p.in_len, first_m, oframes, out);
-				else if (w == 2) LAUNCH((k_rs_mma<2>), grid, 64, 0, st, d_ring, ring_len, C, d_G, g_stride, g_pad, p.n, p.d, p.in_len, first_m, oframes, out);
-				else LAUNCH((k_rs_mma<1>), grid, 32, 0, st, d_ring, ring_len, C, d_G, g_stride, g_pad, p.n, p.d, p.in_len, first_m, oframes, out);
+				if (w == 4) LAUNCH((k_rs_mma<4>), grid, 128, 0, st, d_ring, ring_len, C, d_G, g_stride, g_pad, p.n, p.d, p.in_len, first_m, oframes, out, out16);
+				else if (w == 2) LAUNCH((k_rs_mma<2>), grid, 64, 0, st, d_ring, ring_len, C, d_G, g_stride, g_pad, p.n, p.d, p.in_len, first_m, oframes, out, out16);
+				else LAUNCH((k_rs_mma<1>), grid, 32, 0, st, d_ring, ring_len, C, d_G, g_stride, g_pad, p.n, p.d, p.in_len, first_m, oframes, out, out16);
 				last_kernel = "k_rs_mma";
 				last_warps = w;
 				last_depth = 1;
 			}
 			else {
-				if (tile == 1) rs_launch<16, 4, 4, 2>(st, d_ring, ring_len, C, d_G, g_stride, g_pad, p, first_m, oframes, out);
-				else if (tile == 2) rs_launch<16, 2, 2, 6>(st, d_ring, ring_len, C, d_G, g_stride, g_pad, p, first_m, oframes, out);
-				else rs_launch<8, 1, 4, 4>(st, d_ring, ring_len, C, d_G, g_stride, g_pad, p, first_m, oframes, out);
+				if (tile == 1) rs_launch<16, 4, 4, 2>(st, d_ring, ring_len, C, d_G, g_stride, g_pad, p, first_m, oframes, out, out16);
+				else if (tile == 2) rs_launch<16, 2, 2, 6>(st, d_ring, ring_len, C, d_G, g_stride, g_pad, p, first_m, oframes, out, out16);
+				else rs_launch<8, 1, 4, 4>(st, d_ring, ring_len, C, d_G, g_stride, g_pad, p, first_m, oframes, out, out16);
 				last_kernel = "k_rs_poly";
 				last_warps = (tile == 2) ? 2 : 4;
 				last_depth = 0;

@@ -129,7 +129,15 @@ int  dspb200_chain_wait(dspb200_chain *c, unsigned long long ticket);
  * enqueued on `stream` (a cudaStream_t; NULL = the legacy default stream), asynchronous.
  * d_in == d_out is allowed unless the chain's last operator changes the frame count (resample, align); such a call
  * is rejected before anything runs: it returns < 0 and leaves the buffer and the chain's state as they were.
- * Returns output frames. */
+ * Returns output frames.
+ * Buffers: 8-byte alignment (that of a double) is enough for d_in and d_out; 16-byte-aligned rows may be faster.
+ * d_in is never written unless the call is in place, and of d_out only the returned frames' rows are written.
+ * Streams: every launch of the call waits for the work enqueued on `stream` before it, and `stream` waits for every
+ * launch that reads d_in or writes d_out, so the caller may reuse both buffers in stream order as soon as the call
+ * returns.  The results do not depend on the stream.  Calls of one chain made on different streams must be ordered by
+ * the caller (an event recorded after one call, waited for before the next).  dspb200_chain_reset, _sync, _drain_host
+ * and the host-buffer calls run on the library's own streams and are NOT ordered against Mode D work: synchronise
+ * the device (or the streams of the Mode D calls) before making them. */
 long dspb200_chain_run_device(dspb200_chain *c, int shard, long frames, const double *d_in,
                               double *d_out, void *stream);
 

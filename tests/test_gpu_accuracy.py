@@ -256,8 +256,7 @@ def test_fir_plan_edges_exact(gpu_lib, case, mix):
 def test_fir_cluster_form_falls_back_on_misaligned_device_buffers(gpu_lib, B, P):
     """run_device on torch buffers: whole blocks on 16-byte aligned rows take the cluster form; one whole block and
     two ragged calls on buffers offset by one double (8-byte aligned) take the per-channel form, the stash and the head
-    kernel, which touch the caller's rows with 8-byte accesses only; the stream stays exact.  (A chain holding only this
-    FIR: the resampler stores double2 into the caller's output and does not fall back.)"""
+    kernel, which touch the caller's rows with 8-byte accesses only; the stream stays exact."""
     import torch
     C, T = 8, (P - 1) * B + 1
     rng = np.random.default_rng(B + P)
