@@ -9,6 +9,7 @@
 // concurrently.  There is no cross-shard data dependency, hence no collective.
 #include "common.cuh"
 #include "ops.h"
+#include "resample_plan.h"
 #include "fft.cuh"
 #include "../../include/dsp_b200.h"
 #include <cassert>
@@ -898,7 +899,7 @@ int dspb200_hilbert_taps(long taps, double angle, double *h)
 int dspb200_resample_params(int fs_in, int fs_out, double bandwidth, long out[8])
 {
 	ResampleParams p;
-	if (resample_params(fs_in, fs_out, bandwidth, &p)) return -1;
+	if (resample_params_or_error(fs_in, fs_out, bandwidth, &p)) return -1;
 	out[0] = p.n; out[1] = p.d; out[2] = p.m; out[3] = p.in_len; out[4] = p.out_len;
 	out[5] = p.sinc_len; out[6] = p.out_delay; out[7] = p.in_len;
 	return 0;

@@ -19,11 +19,9 @@ Op *make_align_op(int slab_channels, int fs, const long *delay, long discard_fra
 // resample.c
 Op *make_resample_op(int slab_channels, int fs_in, int fs_out, double bandwidth, cudaStream_t st);
 
-struct ResampleParams {
-	int n, d, m, in_len, out_len, sinc_len, out_delay, sinc_os, m_os;
-	double fc_os;
-};
-int resample_params(int fs_in, int fs_out, double bw, ResampleParams *p);
+// resample_params() (resample_plan.h), which sets the library's error message when the rates or bandwidth are refused
+struct ResampleParams;
+int resample_params_or_error(int fs_in, int fs_out, double bw, ResampleParams *p);
 
 void fir_debug_serialize(int on);
 int test_rfft(int B, int n_ch, const double *d_in, double *d_spec, cudaStream_t st);

@@ -17,62 +17,22 @@
 // 44100->48000) is built on the device at init from the reference's own sinc samples; the hot
 // kernel is a per-channel dot product with lanes along channels, so every load of the
 // interleaved input is a coalesced row and the taps are broadcast loads from shared memory.
-// The reference's per-call frame pacing is replayed by an integer state machine on the host,
-// so each call emits exactly the frame count resample_effect_run() would.
+// The reference's per-call frame pacing is replayed by an integer state machine on the host
+// (RsPacing, resample_plan.h), so each call emits exactly the frame count resample_effect_run() would.
 #include "common.cuh"
 #include "ops.h"
+#include "resample_plan.h"
 #include <cmath>
 
 namespace dspb200 {
 
-static long next_smooth7(long n)
+// resample_params() (resample_plan.h) with the library's message on failure
+int resample_params_or_error(int fs_in, int fs_out, double bw, ResampleParams *p)
 {
-	for (;; ++n) {
-		long m = n;
-		for (int p : { 2, 3, 5, 7 })
-			while (m % p == 0) m /= p;
-		if (m == 1) return n;
-	}
-}
-
-static int gcd_int(int a, int b)
-{
-	while (b) { const int c = a % b; a = b; b = c; }
-	return a;
-}
-
-#define ALBRECHT_M_FACT 17.7822
-
-// resample.c:274-316
-int resample_params(int fs_in, int fs_out, double bw, ResampleParams *p)
-{
-	if (fs_in <= 0 || fs_out <= 0 || fs_in == fs_out) { set_error("resample: bad rates %d -> %d", fs_in, fs_out); return -1; }
-	if (bw == 0.0) bw = 0.939;
-	if (!(bw >= 0.7 && bw <= 0.999)) { set_error("resample: bandwidth out of range"); return -1; }
-	const int max_rate = (fs_out > fs_in) ? fs_out : fs_in, min_rate = (fs_out > fs_in) ? fs_in : fs_out;
-	const int g = gcd_int(fs_out, fs_in);
-	p->n = fs_out / g;
-	p->d = fs_in / g;
-	const int max_factor = (p->n > p->d) ? p->n : p->d, min_factor = (p->n > p->d) ? p->d : p->n;
-	p->m = (int) lround(2.0 * ALBRECHT_M_FACT * max_rate / (min_rate * (1.0 - bw)));
-	const double width = ALBRECHT_M_FACT * max_rate / p->m;
-	const double fc = (min_rate - width) / max_rate;
-	p->sinc_os = (min_factor < 2) ? min_factor : 2;
-	p->fc_os = fc / p->sinc_os;
-	p->m_os = (p->m + 1) * p->sinc_os - 1;
-	int len_mult = (p->m + 1) / max_factor;
-	if ((p->m + 1) % max_factor != 0) len_mult += 1;
-	if (len_mult > 16) {
-		const int fast = (int) next_smooth7(len_mult);
-		if (fast != len_mult && (p->n <= 16 || p->d <= 16 || next_smooth7(p->n) == p->n || next_smooth7(p->d) == p->d))
-			len_mult = fast;
-	}
-	p->sinc_len = max_factor * len_mult * p->sinc_os;
-	p->in_len = p->d * len_mult;
-	p->out_len = p->n * len_mult;
-	if (fs_out == max_rate) p->out_delay = p->m / 2;
-	else p->out_delay = (int) lround(p->m / 2 * ((double) p->n / p->d));
-	return 0;
+	const int e = resample_params(fs_in, fs_out, bw, p);
+	if (e == RS_BAD_RATES) set_error("resample: bad rates %d -> %d", fs_in, fs_out);
+	else if (e == RS_BAD_BANDWIDTH) set_error("resample: bandwidth out of range");
+	return e ? -1 : 0;
 }
 
 // resample.c:52-80 (WINDOW_FUNCTION 3)
@@ -192,6 +152,27 @@ __device__ __forceinline__ void rs_store4(double *o, bool out16, double a, doubl
 	rs_store2(o + 2, out16, c, d);
 }
 
+// The input rows the tile of Q outputs from q0 reads: down from i_top, the window end of its last output (q clamped: a
+// partial last tile repeats the last frame's work and does not store it), k_end rows to the window start of its first.
+struct RsSpan { long i_top; int k_end; };
+template <int Q> __device__ __forceinline__ RsSpan rs_span(long q0, long m0, long n_out, int n, int d, int in_len)
+{
+	const long q_last = (q0 + Q - 1 < n_out) ? q0 + Q - 1 : n_out - 1;
+	const long i_top = ((m0 + q_last) * d) / n;
+	long i_bot = ((m0 + q0) * d) / n - in_len + 1;
+	if (i_bot < 0) i_bot = 0;   // rows before the stream start are zero
+	return { i_top, (int) (i_top - i_bot + 1) };
+}
+
+// Where in G the taps of output q start: its phase's row, at the tap it applies to input row i_top (the index may be
+// <= 0: left pad of G's rows); q clamped like the span's last output.
+__device__ __forceinline__ long rs_tap_row(long q, long m0, long n_out, int n, int d, int g_stride, int pad, long i_top)
+{
+	if (q >= n_out) q = n_out - 1;
+	const long md = (m0 + q) * d, ih = md / n;
+	return (md - ih * n) * g_stride + pad + (ih - i_top);
+}
+
 template <int R, int CH, int WARPS, int MINB>
 __global__ void __launch_bounds__(32 * WARPS, MINB) k_rs_poly(const double *__restrict__ ring, long ring_len, int C, const double *__restrict__ G,
                                                               int g_stride, int pad, int n, int d, int in_len, long m0, long n_out, double *__restrict__ out,
@@ -203,13 +184,7 @@ __global__ void __launch_bounds__(32 * WARPS, MINB) k_rs_poly(const double *__re
 	const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
 	const int c0 = (blockIdx.y * 32 + lane) * CH;
 	const long q0 = (long) blockIdx.x * Q;
-	// first and last output of the tile fix the span of input rows (q clamped: a partial last tile repeats
-	// the last frame's work and does not store it)
-	const long q_last = (q0 + Q - 1 < n_out) ? q0 + Q - 1 : n_out - 1;
-	const long i_top = ((m0 + q_last) * d) / n;
-	long i_bot = ((m0 + q0) * d) / n - in_len + 1;
-	if (i_bot < 0) i_bot = 0;   // rows before the stream start are zero
-	const int k_end = (int) (i_top - i_bot + 1);
+	const auto [i_top, k_end] = rs_span<Q>(q0, m0, n_out, n, d, in_len);
 	double acc[R][CH];
 #pragma unroll
 	for (int r = 0; r < R; ++r)
@@ -226,10 +201,7 @@ __global__ void __launch_bounds__(32 * WARPS, MINB) k_rs_poly(const double *__re
 		// one row of G (coalesced) and stores them down a column of S
 		if (kk > 0) __syncthreads();
 		for (int fr = warp; fr < Q; fr += WARPS) {
-			long q = q0 + fr;
-			if (q >= n_out) q = n_out - 1;
-			const long md = (m0 + q) * d, ih = md / n;
-			const double *gsrc = G + (md - ih * n) * g_stride + pad + (ih - i_top) + kk;   // tap for row i_top - kk
+			const double *gsrc = G + rs_tap_row(q0 + fr, m0, n_out, n, d, g_stride, pad, i_top) + kk;   // tap for row i_top - kk
 #pragma unroll
 			for (int k = lane; k < ROWS; k += 32) S[k * LD + fr] = (kk + k < k_end) ? __ldg(gsrc + k) : 0.0;
 		}
@@ -289,24 +261,57 @@ __device__ __forceinline__ void dmma884(double (&c)[2], double a, double b)
 	asm("mma.sync.aligned.m8n8k4.row.col.f64.f64.f64.f64 {%0,%1}, {%2}, {%3}, {%0,%1};" : "+d"(c[0]), "+d"(c[1]) : "d"(a), "d"(b));
 }
 
-constexpr int RSM_Q = 32, RSM_LD = 40, RSM_ROWS = 128;
+constexpr int RSM_Q = 32, RSM_LD = 40, RSM_ROWS = 128, RSM_MT = 4, RSM_NT = 4;
+
+// B operand of one step: 4 adjacent channels of ring row `row` as two 128-bit loads; the row then moves down the 4
+// rows of the step (k = 4), wrapping around the ring
+__device__ __forceinline__ void rs_load_b(double (&b)[RSM_NT], const double *col, long &row, long ring_len, int C)
+{
+	const double *p = col + row * C;
+	const double2 u = *reinterpret_cast<const double2 *>(p), v = *reinterpret_cast<const double2 *>(p + 2);
+	b[0] = u.x; b[1] = u.y; b[2] = v.x; b[3] = v.y;
+	row -= 4;
+	if (row < 0) row += ring_len;
+}
+// A fragments of step st of a tap tile S (rows 4 st .. 4 st + 3), then the step's MT x NT DMMAs.  The kernels hold the
+// fragments: with them inside one helper, ptxas assigns k_rs_mma's registers differently.
+__device__ __forceinline__ void rs_load_a(double (&a)[RSM_MT], const double *S, int st, int g, int t)
+{
+#pragma unroll
+	for (int mt = 0; mt < RSM_MT; ++mt) a[mt] = S[(4 * st + t) * RSM_LD + 8 * mt + g];
+}
+__device__ __forceinline__ void rs_dmma_step(double (&acc)[RSM_MT][RSM_NT][2], const double (&a)[RSM_MT], const double (&b)[RSM_NT])
+{
+#pragma unroll
+	for (int mt = 0; mt < RSM_MT; ++mt)
+#pragma unroll
+		for (int j = 0; j < RSM_NT; ++j) dmma884(acc[mt][j], a[mt], b[j]);
+}
+// D fragment: row lane/4, columns 2 t and 2 t + 1 of n-tile j = channels c0w + 8 t + j and c0w + 8 t + 4 + j
+__device__ __forceinline__ void rs_dmma_store(const double (&acc)[RSM_MT][RSM_NT][2], double *out, bool out16, long q0, long n_out, int C, int c0w, int g, int t)
+{
+	const int ch = c0w + 8 * t;
+#pragma unroll
+	for (int mt = 0; mt < RSM_MT; ++mt) {
+		const long q = q0 + 8 * mt + g;
+		if (q >= n_out) continue;
+		double *o = out + q * C + ch;
+		if (ch < C) rs_store4(o, out16, acc[mt][0][0], acc[mt][1][0], acc[mt][2][0], acc[mt][3][0]);
+		if (ch + 4 < C) rs_store4(o + 4, out16, acc[mt][0][1], acc[mt][1][1], acc[mt][2][1], acc[mt][3][1]);
+	}
+}
 
 template <int WARPS>
 __global__ void __launch_bounds__(32 * WARPS, (WARPS == 4) ? 4 : 1) k_rs_mma(const double *__restrict__ ring, long ring_len, int C, const double *__restrict__ G,
                                                        int g_stride, int pad, int n, int d, int in_len, long m0, long n_out, double *__restrict__ out,
                                                        bool out16)
 {
-	constexpr int MT = 4, NT = 4, Q = RSM_Q, LD = RSM_LD, ROWS = RSM_ROWS;
+	constexpr int MT = RSM_MT, NT = RSM_NT, Q = RSM_Q, LD = RSM_LD, ROWS = RSM_ROWS;
 	__shared__ __align__(16) double S[ROWS * LD];
-	const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-	const int g = lane >> 2, t = lane & 3;
+	const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5, g = lane >> 2, t = lane & 3;
 	const int c0w = (blockIdx.y * WARPS + warp) * 32;
 	const long q0 = (long) blockIdx.x * Q;
-	const long q_last = (q0 + Q - 1 < n_out) ? q0 + Q - 1 : n_out - 1;
-	const long i_top = ((m0 + q_last) * d) / n;
-	long i_bot = ((m0 + q0) * d) / n - in_len + 1;
-	if (i_bot < 0) i_bot = 0;   // rows before the stream start are zero
-	const int k_end = (int) (i_top - i_bot + 1);
+	const auto [i_top, k_end] = rs_span<Q>(q0, m0, n_out, n, d, in_len);
 	double acc[MT][NT][2];
 #pragma unroll
 	for (int mt = 0; mt < MT; ++mt)
@@ -318,32 +323,19 @@ __global__ void __launch_bounds__(32 * WARPS, (WARPS == 4) ? 4 : 1) k_rs_mma(con
 	long row = (i_top - t) % ring_len;
 	if (row < 0) row += ring_len;
 	double bn[NT];
-	{
-		const double *p = col + row * C;
-		const double2 u = *reinterpret_cast<const double2 *>(p), v = *reinterpret_cast<const double2 *>(p + 2);
-		bn[0] = u.x; bn[1] = u.y; bn[2] = v.x; bn[3] = v.y;
-		row -= 4;
-		if (row < 0) row += ring_len;
-	}
+	rs_load_b(bn, col, row, ring_len, C);
 	for (int kk = 0; kk < k_end; kk += ROWS) {
 		if (kk > 0) __syncthreads();
-		{
-			// gather: this lane fills columns g, g + 8, g + 16, g + 24 of S, rows k = 4 kg + t (the pointers are
-			// rebuilt per chunk rather than kept in registers through the multiply loop)
-			const double *gs[MT];
+		// gather: this lane fills columns g, g + 8, g + 16, g + 24 of S, rows k = 4 kg + t (the pointers are
+		// rebuilt per chunk rather than kept in registers through the multiply loop)
+		const double *gs[MT];
 #pragma unroll
-			for (int m = 0; m < MT; ++m) {
-				long q = q0 + g + 8 * m;
-				if (q >= n_out) q = n_out - 1;
-				const long md = (m0 + q) * d, ih = md / n;
-				gs[m] = G + (md - ih * n) * g_stride + pad + (ih - i_top) + kk;   // tap of row i_top - kk (index may be <= 0: left pad)
-			}
-			for (int kg = warp; kg < ROWS / 4; kg += WARPS) {
-				const int k = 4 * kg + t;
-				const bool in = kk + k < k_end;
+		for (int m = 0; m < MT; ++m) gs[m] = G + rs_tap_row(q0 + g + 8 * m, m0, n_out, n, d, g_stride, pad, i_top) + kk;   // tap of row i_top - kk
+		for (int kg = warp; kg < ROWS / 4; kg += WARPS) {
+			const int k = 4 * kg + t;
+			const bool in = kk + k < k_end;
 #pragma unroll
-				for (int m = 0; m < MT; ++m) S[k * LD + g + 8 * m] = in ? __ldg(gs[m] + k) : 0.0;
-			}
+			for (int m = 0; m < MT; ++m) S[k * LD + g + 8 * m] = in ? __ldg(gs[m] + k) : 0.0;
 		}
 		__syncthreads();
 		const int left = k_end - kk;
@@ -352,32 +344,13 @@ __global__ void __launch_bounds__(32 * WARPS, (WARPS == 4) ? 4 : 1) k_rs_mma(con
 			double b[NT];
 #pragma unroll
 			for (int j = 0; j < NT; ++j) b[j] = bn[j];
-			{
-				const double *p = col + row * C;
-				const double2 u = *reinterpret_cast<const double2 *>(p), v = *reinterpret_cast<const double2 *>(p + 2);
-				bn[0] = u.x; bn[1] = u.y; bn[2] = v.x; bn[3] = v.y;
-				row -= 4;
-				if (row < 0) row += ring_len;
-			}
+			rs_load_b(bn, col, row, ring_len, C);
 			double a[MT];
-#pragma unroll
-			for (int mt = 0; mt < MT; ++mt) a[mt] = S[(4 * st + t) * LD + 8 * mt + g];
-#pragma unroll
-			for (int mt = 0; mt < MT; ++mt)
-#pragma unroll
-				for (int j = 0; j < NT; ++j) dmma884(acc[mt][j], a[mt], b[j]);
+			rs_load_a(a, S, st, g, t);
+			rs_dmma_step(acc, a, b);
 		}
 	}
-	// D fragment: row lane/4, columns 2 t and 2 t + 1 of n-tile j = channels c0w + 8 t + j and c0w + 8 t + 4 + j
-	const int ch = c0w + 8 * t;
-#pragma unroll
-	for (int mt = 0; mt < MT; ++mt) {
-		const long q = q0 + 8 * mt + g;
-		if (q >= n_out) continue;
-		double *o = out + q * C + ch;
-		if (ch < C) rs_store4(o, out16, acc[mt][0][0], acc[mt][1][0], acc[mt][2][0], acc[mt][3][0]);
-		if (ch + 4 < C) rs_store4(o + 4, out16, acc[mt][0][1], acc[mt][1][1], acc[mt][2][1], acc[mt][3][1]);
-	}
+	rs_dmma_store(acc, out, out16, q0, n_out, C, c0w, g, t);
 }
 
 // The same kernel with the tap tile double-buffered: the gather of chunk k+1 (cp.async, 8 bytes each, straight into
@@ -385,7 +358,6 @@ __global__ void __launch_bounds__(32 * WARPS, (WARPS == 4) ? 4 : 1) k_rs_mma(con
 // barrier per chunk instead of a gather phase in which the CTA's four warps issue no DMMA at all.  Chunks of 64 rows: the two halves together are the 40 KB of
 // the single-buffered form, four CTAs per SM as before.
 constexpr int RSM2_ROWS = 64;
-constexpr int RS_DEFAULT_MMA = 7;   // 4: single-buffered tap tile; 7: double-buffered, input rows two steps ahead, 3 CTAs per SM (no spills)
 
 __device__ __forceinline__ void cp_async8(double *smem_dst, const double *gsrc, bool valid)
 {
@@ -401,32 +373,23 @@ __global__ void __launch_bounds__(32 * WARPS, MINB) k_rs_mma2(const double *__re
                                                         int g_stride, int pad, int n, int d, int in_len, long m0, long n_out, double *__restrict__ out,
                                                         bool out16)
 {
-	constexpr int MT = 4, NT = 4, Q = RSM_Q, LD = RSM_LD, ROWS = RSM2_ROWS;
+	constexpr int MT = RSM_MT, NT = RSM_NT, Q = RSM_Q, LD = RSM_LD, ROWS = RSM2_ROWS;
 	__shared__ __align__(16) double S[2][ROWS * LD];
-	const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-	const int g = lane >> 2, t = lane & 3;
+	const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5, g = lane >> 2, t = lane & 3;
 	const int c0w = (blockIdx.y * WARPS + warp) * 32;
 	const long q0 = (long) blockIdx.x * Q;
-	const long q_last = (q0 + Q - 1 < n_out) ? q0 + Q - 1 : n_out - 1;
-	const long i_top = ((m0 + q_last) * d) / n;
-	long i_bot = ((m0 + q0) * d) / n - in_len + 1;
-	if (i_bot < 0) i_bot = 0;   // rows before the stream start are zero
-	const int k_end = (int) (i_top - i_bot + 1);
+	const RsSpan span = rs_span<Q>(q0, m0, n_out, n, d, in_len);   // not bound to names: gather() captures k_end
+	const long i_top = span.i_top; const int k_end = span.k_end;
 	double acc[MT][NT][2];
 #pragma unroll
 	for (int mt = 0; mt < MT; ++mt)
 #pragma unroll
 		for (int j = 0; j < NT; ++j) acc[mt][j][0] = acc[mt][j][1] = 0.0;
 	// this lane fills columns g, g + 8, g + 16, g + 24 of S, rows k = 4 kg + t: tap of row i_top - k of the output
-	// frame's phase (the index may be <= 0: left pad of G's rows)
+	// frame's phase
 	long goff[MT];
 #pragma unroll
-	for (int m = 0; m < MT; ++m) {
-		long q = q0 + g + 8 * m;
-		if (q >= n_out) q = n_out - 1;
-		const long md = (m0 + q) * d, ih = md / n;
-		goff[m] = (md - ih * n) * g_stride + pad + (ih - i_top);
-	}
+	for (int m = 0; m < MT; ++m) goff[m] = rs_tap_row(q0 + g + 8 * m, m0, n_out, n, d, g_stride, pad, i_top);
 	auto gather = [&](int kk, double *Sb) {
 		for (int kg = warp; kg < ROWS / 4; kg += WARPS) {
 			const int k = 4 * kg + t;
@@ -444,19 +407,12 @@ __global__ void __launch_bounds__(32 * WARPS, MINB) k_rs_mma2(const double *__re
 	if (row < 0) row += ring_len;
 	double bq[DEPTH][NT];
 #pragma unroll
-	for (int dd = 0; dd < DEPTH; ++dd) {
-		const double *p = col + row * C;
-		const double2 u = *reinterpret_cast<const double2 *>(p), v = *reinterpret_cast<const double2 *>(p + 2);
-		bq[dd][0] = u.x; bq[dd][1] = u.y; bq[dd][2] = v.x; bq[dd][3] = v.y;
-		row -= 4;
-		if (row < 0) row += ring_len;
-	}
+	for (int dd = 0; dd < DEPTH; ++dd) rs_load_b(bq[dd], col, row, ring_len, C);
 	asm volatile("cp.async.wait_group 0;" ::: "memory");
 	__syncthreads();
 	int cur = 0;
 	for (int kk = 0; kk < k_end; kk += ROWS) {
 		if (kk + ROWS < k_end) gather(kk + ROWS, S[cur ^ 1]);   // nobody reads that half any more (barrier below)
-		const double *Sc = S[cur];
 		const int left = k_end - kk;
 		const int steps = (left < ROWS) ? (left + 3) / 4 : ROWS / 4;
 		for (int st = 0; st < steps; ++st) {
@@ -467,45 +423,33 @@ __global__ void __launch_bounds__(32 * WARPS, MINB) k_rs_mma2(const double *__re
 			for (int dd = 0; dd + 1 < DEPTH; ++dd)
 #pragma unroll
 				for (int j = 0; j < NT; ++j) bq[dd][j] = bq[dd + 1][j];
-			{
-				const double *p = col + row * C;
-				const double2 u = *reinterpret_cast<const double2 *>(p), v = *reinterpret_cast<const double2 *>(p + 2);
-				bq[DEPTH - 1][0] = u.x; bq[DEPTH - 1][1] = u.y; bq[DEPTH - 1][2] = v.x; bq[DEPTH - 1][3] = v.y;
-				row -= 4;
-				if (row < 0) row += ring_len;
-			}
+			rs_load_b(bq[DEPTH - 1], col, row, ring_len, C);
 			double a[MT];
-#pragma unroll
-			for (int mt = 0; mt < MT; ++mt) a[mt] = Sc[(4 * st + t) * LD + 8 * mt + g];
-#pragma unroll
-			for (int mt = 0; mt < MT; ++mt)
-#pragma unroll
-				for (int j = 0; j < NT; ++j) dmma884(acc[mt][j], a[mt], b[j]);
+			rs_load_a(a, S[cur], st, g, t);
+			rs_dmma_step(acc, a, b);
 		}
 		asm volatile("cp.async.wait_group 0;" ::: "memory");
 		__syncthreads();   // the next half is complete and visible; this half is free
 		cur ^= 1;
 	}
-	// D fragment: row lane/4, columns 2 t and 2 t + 1 of n-tile j = channels c0w + 8 t + j and c0w + 8 t + 4 + j
-	const int ch = c0w + 8 * t;
-#pragma unroll
-	for (int mt = 0; mt < MT; ++mt) {
-		const long q = q0 + 8 * mt + g;
-		if (q >= n_out) continue;
-		double *o = out + q * C + ch;
-		if (ch < C) rs_store4(o, out16, acc[mt][0][0], acc[mt][1][0], acc[mt][2][0], acc[mt][3][0]);
-		if (ch + 4 < C) rs_store4(o + 4, out16, acc[mt][0][1], acc[mt][1][1], acc[mt][2][1], acc[mt][3][1]);
-	}
+	rs_dmma_store(acc, out, out16, q0, n_out, C, c0w, g, t);
 }
 
-template <int R, int CH, int WARPS, int MINB>
-static void rs_launch(cudaStream_t st, const double *ring, long ring_len, int C, const double *G, int g_stride, int pad,
-                      const ResampleParams &p, long m0, long n_out, double *out, bool out16)
+using RsKernel = void (*)(const double *, long, int, const double *, int, int, int, int, int, long, long, double *, bool);
+// The instantiation that runs a launch, its template arguments read from rs_variant() (resample_plan.h), so that
+// describe() reports what ran.  The FMA tiles have fixed warps: rs_instance<T, W> is the same kernel for every W.
+template <int T, int W> static RsKernel rs_instance()
 {
-	using Cfg = RsCfg<R, CH, WARPS>;
-	const dim3 grid((unsigned) ceil_div(n_out, Cfg::Q), (unsigned) ceil_div(C, 32 * CH));
-	LAUNCH((k_rs_poly<R, CH, WARPS, MINB>), grid, Cfg::THREADS, 0, st, ring, ring_len, C, G, g_stride, pad, p.n, p.d, p.in_len, m0, n_out, out, out16);
+	constexpr RsLaunch v = rs_variant(T, W);
+	static_assert((T <= 3) ? v.Q % v.warps == 0 && v.channels % 32 == 0 : v.Q == RSM_Q && v.channels == 32 * W, "variant's tile");
+	static_assert(T != 4 || v.minb == ((W == 4) ? 4 : 1), "k_rs_mma's launch bounds");
+	if constexpr (T <= 3) return k_rs_poly<v.Q / v.warps, v.channels / 32, v.warps, v.minb>;
+	else if constexpr (T == 4) return k_rs_mma<W>;
+	else return k_rs_mma2<W, v.minb, v.depth>;
 }
+template <int T> static RsKernel rs_tile_kernel(int w) { return (w == 4) ? rs_instance<T, 4>() : (w == 2) ? rs_instance<T, 2>() : rs_instance<T, 1>(); }
+static RsKernel (*const rs_kernel[8])(int warps) = { nullptr, rs_tile_kernel<1>, rs_tile_kernel<2>, rs_tile_kernel<3>, rs_tile_kernel<4>,
+                                                     rs_tile_kernel<5>, rs_tile_kernel<6>, rs_tile_kernel<7> };   // by tile
 
 // move the live rows of the input ring into a bigger ring (absolute frame a lives at a % len)
 __global__ void k_rs_ring_grow(const double *old_ring, long old_len, double *new_ring, long new_len, int C, long a0, long rows)
@@ -518,24 +462,14 @@ __global__ void k_rs_ring_grow(const double *old_ring, long old_len, double *new
 }
 
 struct ResampleOp : Op {
-	ResampleParams p;
+	RsPacing pace;
+	const ResampleParams &p = pace.p;
 	double *d_G = nullptr, *d_ring = nullptr;
 	int g_stride = 0, g_pad = 0;         // tap rows: [pad zeros | in_len taps | pad zeros]
-	long ring_len = 0;
-	// resample.c:39-50 bookkeeping (integers only; the sample data lives in the ring)
-	long total_in = 0;          // frames appended since reset
-	long emit_pos = 0;          // next raw output index to emit
-	int in_buf_pos = 0, out_buf_pos = 0, has_output = 0;
-	int is_draining = 0;
-	long drain_pos = 0, drain_frames = 0;
-	// DSP_B200_RS_TILE, read when the operator is made: 0 auto, 1..3 the FMA tiles (16x4, 16x2, 8x1), 4 tensor-core
-	// kernel, 5..7 the same with the tap tile double-buffered (cp.async) and the input rows requested 2 / 3 / 2 steps
-	// ahead at 4 / 3 / 3 CTAs per SM.  A forced tile the channel count cannot use falls back to the default.
-	int force_tile = 0;
-	// the last launch, for describe(): kernel, tile, warps per CTA, input-row steps requested ahead (0: FMA kernel),
-	// alignment of the output in bytes (16: 128-bit stores, 8: 64-bit stores)
-	const char *last_kernel = "";
-	int last_tile = 0, last_warps = 0, last_depth = 0, last_out_align = 0;
+	long ring_len = 0, total_in = 0;   // total_in: frames appended since reset
+	int force_tile = 0;         // DSP_B200_RS_TILE (resample_plan.h), read when the operator is made
+	// the last launch, for describe(), and the alignment of its output in bytes (16: 128-bit stores, 8: 64-bit stores)
+	RsLaunch last; int last_out_align = 0;
 
 	const char *name() const override { return "resample"; }
 
@@ -544,24 +478,17 @@ struct ResampleOp : Op {
 		char buf[384];
 		snprintf(buf, sizeof(buf), "{\"op\":\"resample\",\"n\":%d,\"d\":%d,\"in_len\":%d,\"out_len\":%d,\"out_delay\":%d,\"ring_len\":%ld,"
 		         "\"force_tile\":%d,\"kernel\":\"%s\",\"tile\":%d,\"warps\":%d,\"depth\":%d,\"out_align\":%d}",
-		         p.n, p.d, p.in_len, p.out_len, p.out_delay, ring_len, force_tile, last_kernel, last_tile, last_warps, last_depth, last_out_align);
+		         p.n, p.d, p.in_len, p.out_len, p.out_delay, ring_len, force_tile, last.kernel, last.tile, last.warps, last.depth, last_out_align);
 		return buf;
 	}
 	~ResampleOp() override { dev_free(d_G); dev_free(d_ring); }
 
-	long max_out_frames(long in_frames) const override
-	{
-		const long long r = (long long) in_frames * p.n;
-		return (long) ((r % p.d != 0) ? r / p.d + 1 : r / p.d);
-	}
+	long max_out_frames(long in_frames) const override { return pace.max_out_frames(in_frames); }
 
 	void reset(cudaStream_t st) override
 	{
-		// resample.c:154-161 (the drain counters are deliberately left alone, as there)
-		in_buf_pos = out_buf_pos = 0;
-		has_output = 0;
+		pace.reset();
 		total_in = 0;
-		emit_pos = 0;
 		if (d_ring) cudaMemsetAsync(d_ring, 0, (size_t) ring_len * channels * sizeof(double), st);
 	}
 
@@ -587,8 +514,8 @@ struct ResampleOp : Op {
 	long run(long frames, const double *in, double *out, cudaStream_t st) override
 	{
 		if (frames <= 0) return 0;
-		const int C = channels;
-		if (ensure_ring(frames, st)) return -1;
+		const int C = channels, sms = sm_count();
+		if (sms < 1 || ensure_ring(frames, st)) return -1;
 		// append the new rows (at most one wrap)
 		{
 			const long w = total_in % ring_len;
@@ -598,105 +525,28 @@ struct ResampleOp : Op {
 				CUDA_TRY(cudaMemcpyAsync(d_ring, in + first * C, (size_t) (frames - first) * C * sizeof(double), cudaMemcpyDeviceToDevice, st), return -1);
 			total_in += frames;
 		}
-		// replay resample_effect_run()'s pacing, resample.c:91-151
-		const long max_oframes = max_out_frames(frames);
-		long iframes = 0, oframes = 0;
-		while (iframes < frames) {
-			long take = p.in_len - in_buf_pos;
-			if (take > frames - iframes) take = frames - iframes;
-			in_buf_pos += (int) take;
-			iframes += take;
-			if (has_output) {
-				long emit = p.out_len - out_buf_pos;
-				if (emit > max_oframes - oframes) emit = max_oframes - oframes;
-				out_buf_pos += (int) emit;
-				oframes += emit;
-			}
-			if (in_buf_pos == p.in_len && (!has_output || out_buf_pos == p.out_len)) {
-				in_buf_pos = out_buf_pos = 0;
-				if (!has_output) {
-					out_buf_pos = p.out_delay;
-					emit_pos += p.out_delay;   // only ever happens before the first emitted frame
-					has_output = 1;
-				}
-			}
-			else if (take == 0) {
-				set_error("resample: pacing stalled (in_buf_pos=%d out_buf_pos=%d)", in_buf_pos, out_buf_pos);
-				return -1;
-			}
-		}
-		const long first_m = emit_pos;   // emission is one contiguous raw range per call
-		if (oframes > 0) {
-			ProfScope prof("resample", st);
-			const int force = force_tile;   // 1..7 where the channel count allows it (see force_tile)
-			int tile = (C % 4 == 0) ? RS_DEFAULT_MMA : (C % 2 == 0) ? 2 : 3;
-			if (force >= 1 && force <= 7 && !(((force == 1 || force >= 4) && C % 4) || (force == 2 && C % 2))) tile = force;
-			const long sms = sm_count();   // the tensor-core kernels: warps per CTA as long as every SM still gets a few CTAs
-			if (sms < 1) return -1;
-			last_tile = tile;
-			// the stores into the caller's rows: 128-bit when `out` allows it (a row offset is a multiple of 16 bytes
-			// wherever a kernel stores pairs), else 64-bit -- the same values either way
-			const bool out16 = (reinterpret_cast<uintptr_t>(out) & 15) == 0;
-			last_out_align = out16 ? 16 : 8;
-			if (tile >= 5) {
-				const long tiles = ceil_div(oframes, RSM_Q);
-				const int w = (C >= 128 && tiles * ceil_div(C, 128) >= sms * 3) ? 4 : (C >= 64 && tiles * ceil_div(C, 64) >= sms * 2) ? 2 : 1;
-				const dim3 grid((unsigned) tiles, (unsigned) ceil_div(C, 32 * w));
-#define RS_MMA2(W, MINB, DEPTH) LAUNCH((k_rs_mma2<W, MINB, DEPTH>), grid, 32 * W, 0, st, d_ring, ring_len, C, d_G, g_stride, g_pad, p.n, p.d, p.in_len, first_m, oframes, out, out16)
-				if (w == 4 && tile == 5) RS_MMA2(4, 4, 2);
-				else if (w == 4 && tile == 6) RS_MMA2(4, 3, 3);
-				else if (w == 4) RS_MMA2(4, 3, 2);
-				else if (w == 2) RS_MMA2(2, 1, 2);
-				else RS_MMA2(1, 1, 2);
-#undef RS_MMA2
-				last_kernel = "k_rs_mma2";
-				last_warps = w;
-				last_depth = (w == 4 && tile == 6) ? 3 : 2;
-			}
-			else if (tile == 4) {
-				// 4 warps (128 channels) per CTA when that still gives every SM a few CTAs, else 2 or 1
-				const long tiles = ceil_div(oframes, RSM_Q);
-				const int w = (C >= 128 && tiles * ceil_div(C, 128) >= sms * 3) ? 4 : (C >= 64 && tiles * ceil_div(C, 64) >= sms * 2) ? 2 : 1;
-				const dim3 grid((unsigned) tiles, (unsigned) ceil_div(C, 32 * w));
-				if (w == 4) LAUNCH((k_rs_mma<4>), grid, 128, 0, st, d_ring, ring_len, C, d_G, g_stride, g_pad, p.n, p.d, p.in_len, first_m, oframes, out, out16);
-				else if (w == 2) LAUNCH((k_rs_mma<2>), grid, 64, 0, st, d_ring, ring_len, C, d_G, g_stride, g_pad, p.n, p.d, p.in_len, first_m, oframes, out, out16);
-				else LAUNCH((k_rs_mma<1>), grid, 32, 0, st, d_ring, ring_len, C, d_G, g_stride, g_pad, p.n, p.d, p.in_len, first_m, oframes, out, out16);
-				last_kernel = "k_rs_mma";
-				last_warps = w;
-				last_depth = 1;
-			}
-			else {
-				if (tile == 1) rs_launch<16, 4, 4, 2>(st, d_ring, ring_len, C, d_G, g_stride, g_pad, p, first_m, oframes, out, out16);
-				else if (tile == 2) rs_launch<16, 2, 2, 6>(st, d_ring, ring_len, C, d_G, g_stride, g_pad, p, first_m, oframes, out, out16);
-				else rs_launch<8, 1, 4, 4>(st, d_ring, ring_len, C, d_G, g_stride, g_pad, p, first_m, oframes, out, out16);
-				last_kernel = "k_rs_poly";
-				last_warps = (tile == 2) ? 2 : 4;
-				last_depth = 0;
-			}
-			emit_pos += oframes;
-		}
-		return oframes;
+		const RsCall call = pace.run(frames);   // resample_effect_run()'s pacing
+		if (call.frames < 0) set_error("resample: pacing stalled (in_buf_pos=%d out_buf_pos=%d)", pace.in_buf_pos, pace.out_buf_pos);
+		if (call.frames <= 0) return call.frames;   // -1 when stalled
+		ProfScope prof("resample", st);
+		last = rs_launch(C, call.frames, sms, force_tile);
+		// the stores into the caller's rows: 128-bit when `out` allows it (a row offset is a multiple of 16 bytes
+		// wherever a kernel stores pairs), else 64-bit -- the same values either way
+		const bool out16 = (reinterpret_cast<uintptr_t>(out) & 15) == 0;
+		last_out_align = out16 ? 16 : 8;
+		const dim3 grid((unsigned) ceil_div(call.frames, last.Q), (unsigned) ceil_div(C, last.channels));
+		LAUNCH(rs_kernel[last.tile](last.warps), grid, 32 * last.warps, 0, st, d_ring, ring_len, C, d_G, g_stride, g_pad, p.n, p.d, p.in_len, call.first, call.frames,
+		       out, out16);
+		return call.frames;
 	}
 
 	// resample.c:163-188
 	long drain2(long frames, double *zeros, double *out, cudaStream_t st) override
 	{
-		if (!has_output && in_buf_pos == 0) return -1;
-		if (!is_draining) {
-			if (has_output) {
-				drain_frames += p.out_delay;
-				drain_frames += p.out_len - out_buf_pos;
-			}
-			drain_frames += max_out_frames(in_buf_pos);
-			is_draining = 1;
-		}
-		if (drain_pos >= drain_frames) return -1;
+		if (pace.drain_dry()) return -1;
 		CUDA_TRY(cudaMemsetAsync(zeros, 0, (size_t) frames * channels * sizeof(double), st), return -2);
-		long produced = run(frames, zeros, out, st);
-		if (produced < 0) return -2;
-		drain_pos += produced;
-		if (drain_pos > drain_frames) produced -= drain_pos - drain_frames;
-		return produced;
+		const long produced = run(frames, zeros, out, st);
+		return (produced < 0) ? -2 : pace.drain_trim(produced);
 	}
 };
 
@@ -708,7 +558,7 @@ Op *make_resample_op(int slab_channels, int fs_in, int fs_out, double bandwidth,
 	op->fs_out = fs_out;
 	op->inplace_ok = false;
 	op->force_tile = getenv("DSP_B200_RS_TILE") ? atoi(getenv("DSP_B200_RS_TILE")) : 0;
-	if (resample_params(fs_in, fs_out, bandwidth, &op->p)) return nullptr;
+	if (resample_params_or_error(fs_in, fs_out, bandwidth, &op->pace.p)) return nullptr;
 	const ResampleParams &p = op->p;
 
 	// windowed sinc, resample.c:361-364 (host libm, like the reference)

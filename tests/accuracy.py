@@ -312,7 +312,8 @@ CSRC = os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file__))),
 
 
 def header_lib(tmp_dir, name, source):
-    """Compile a C++ driver of the host-only header dsp_b200/csrc/fir_plan.h with g++ alone (no CUDA); -> ctypes.CDLL."""
+    """Compile a C++ driver of a host-only header of dsp_b200/csrc (fir_plan.h, resample_plan.h) with g++ alone (no
+    CUDA); -> ctypes.CDLL."""
     src, so = tmp_dir / (name + ".cpp"), tmp_dir / ("lib%s.so" % name)
     src.write_text(source)
     subprocess.run(["g++", "-std=c++17", "-O1", "-Wall", "-Werror", "-shared", "-fPIC", "-I", CSRC, str(src), "-o", str(so)], check=True)
@@ -512,9 +513,28 @@ def fir_nan_window(n, taps, levels, latency=0):
     return n // B0 * B0 + latency, n + taps + 2 * Bl + latency
 
 
-# Output frames per CTA of each resampler variant (DSP_B200_RS_TILE): RsCfg<R, CH, WARPS>::Q = R WARPS of the FMA
-# kernel's instantiations (tile 1: 16 x 4 warps, 2: 16 x 2, 3: 8 x 4) and RSM_Q of the tensor-core kernels (resample.cu).
-RS_TILE_Q = {1: 64, 2: 32, 3: 32, 4: 32, 5: 32, 6: 32, 7: 32}
+def rs_expect_launch(C, force, oframes, sms):
+    """The launch of a resampler call that emits `oframes` frames on C channels, with DSP_B200_RS_TILE=`force` (0:
+    unset), on a device of `sms` SMs -- rs_launch() of dsp_b200/csrc/resample_plan.h, restated.  Tiles 1..3 are the FMA
+    kernel's R x CH register tiles on a fixed number of warps; 4 is the tensor-core kernel, 5..7 its double-buffered
+    form (7 is the default wherever C % 4 == 0, else 2 on even C, else 3; a forced tile the channel count cannot use
+    falls back to it).  The tensor-core kernels take 4 warps (128 channels) per CTA while that still leaves 3 CTAs per SM,
+    else 2 warps while that leaves 2, else 1.  depth: input-row steps requested ahead (0 on the FMA kernel); minb: CTAs
+    per SM of the instantiation's launch bounds; Q: output frames per CTA; channels: channels per CTA."""
+    usable = {1: C % 4 == 0, 2: C % 2 == 0, 3: True, 4: C % 4 == 0, 5: C % 4 == 0, 6: C % 4 == 0, 7: C % 4 == 0}
+    tile = force if usable.get(force, False) else 7 if C % 4 == 0 else 2 if C % 2 == 0 else 3
+    fma = {1: (16, 4, 4, 2), 2: (16, 2, 2, 6), 3: (8, 1, 4, 4)}   # R, CH, warps, minb of k_rs_poly
+    if tile in fma:
+        R, CH, warps, minb = fma[tile]
+        return dict(tile=tile, kernel="k_rs_poly", warps=warps, depth=0, minb=minb, Q=R * warps, channels=32 * CH)
+    ctas = lambda w: -(-oframes // 32) * -(-C // (32 * w))
+    warps = 4 if C >= 128 and ctas(4) >= 3 * sms else 2 if C >= 64 and ctas(2) >= 2 * sms else 1
+    if tile == 4:
+        kernel, depth, minb = "k_rs_mma", 1, 4 if warps == 4 else 1
+    else:
+        kernel, depth = "k_rs_mma2", 3 if tile == 6 and warps == 4 else 2
+        minb = {5: 4, 6: 3, 7: 3}[tile] if warps == 4 else 1
+    return dict(tile=tile, kernel=kernel, warps=warps, depth=depth, minb=minb, Q=32, channels=32 * warps)
 
 
 def rs_nan_windows(n, counts, n_, d, in_len, out_delay, Q):

@@ -37,7 +37,8 @@ import numpy as np
 import pytest
 
 from accuracy import (F2, F4, FIR_CASES, FIR_EDGES, H_MAX, RS_RATIOS, RsPacing, _fir_plan, _ladder, biquad_within_ref, dyadic_signal,
-                      dyadic_taps, env, exact_conv, fir_nerr, resample_taps_truth, resample_truth, rs_counts, rs_nerr, taps_norm)
+                      dyadic_taps, env, exact_conv, fir_nerr, resample_taps_truth, resample_truth, rs_counts, rs_expect_launch, rs_nerr,
+                      taps_norm)
 
 pytestmark = pytest.mark.gpu
 FIR_RMS, FIR_MAX = 1e-14, 1e-13
@@ -502,19 +503,6 @@ def _plan(ch):
     return p
 
 
-def _expect_tile(C, force):
-    """The variant resample.cu runs for `force` (0: none) on C channels."""
-    tile = 7 if C % 4 == 0 else 2 if C % 2 == 0 else 3
-    if 1 <= force <= 7 and not (((force == 1 or force >= 4) and C % 4) or (force == 2 and C % 2)):
-        tile = force
-    return tile, ("k_rs_poly" if tile <= 3 else "k_rs_mma" if tile == 4 else "k_rs_mma2")
-
-
-def _expect_warps(C, oframes, sms):
-    tiles = -(-oframes // 32)
-    return 4 if C >= 128 and tiles * -(-C // 128) >= 3 * sms else 2 if C >= 64 and tiles * -(-C // 64) >= 2 * sms else 1
-
-
 def rs_bases(fi, fo, bw, N, seed):
     """[N, 5]: dyadic white noise; a 0.9 full-scale sine just inside the passband edge; a tone in the stopband (in the
     transition band when upsampling, where the input has no stopband); a DC step 0 -> 0.9; +-0.5 at the input Nyquist."""
@@ -636,7 +624,8 @@ def test_resample_every_variant_at_channel_tile_edges(gpu_lib, shape):
         x = _tiled(base, C)
         family = {}
         for force in range(8):
-            tile, kernel = _expect_tile(C, force)
+            want = rs_expect_launch(C, force, 1, 1)
+            tile, kernel = want["tile"], want["kernel"]
             ch = _rs_chain(gpu_lib, fi, fo, C, bw, force)
             outs = _run_calls(ch, x, sizes)
             plan = _plan(ch)
@@ -680,10 +669,10 @@ def test_resample_warps_per_cta(gpu_lib, C):
             pos += f
             if outs[-1].shape[0]:
                 plan = _plan(ch)
-                w = _expect_warps(C, outs[-1].shape[0], sms)
-                assert (plan["tile"], plan["warps"]) == (force, w), (force, outs[-1].shape[0], plan)
-                assert plan["depth"] == (1 if force == 4 else 3 if force == 6 and w == 4 else 2), plan
-                reached.add(w)
+                want = rs_expect_launch(C, force, outs[-1].shape[0], sms)
+                assert (plan["tile"], plan["warps"]) == (force, want["warps"]), (force, outs[-1].shape[0], plan)
+                assert plan["depth"] == want["depth"], plan
+                reached.add(want["warps"])
         ch.close()
         assert reached == allowed, (force, reached)
         got = np.concatenate(outs)

@@ -32,8 +32,8 @@ import zlib
 import numpy as np
 import pytest
 
-from accuracy import FIR_CASES, FIR_EDGES, biquad_within_ref, dyadic_signal, env, exact_conv, fir_nerr, rs_counts
-from test_gpu_accuracy import (BQ_SECTIONS, FIR_MAX, FIR_RMS, H_SHIFT, _check_plan, _check_stream, _design, _expect_tile, _expect_warps,
+from accuracy import FIR_CASES, FIR_EDGES, biquad_within_ref, dyadic_signal, env, exact_conv, fir_nerr, rs_counts, rs_expect_launch
+from test_gpu_accuracy import (BQ_SECTIONS, FIR_MAX, FIR_RMS, H_SHIFT, _check_plan, _check_stream, _design,
                                _rs_chain, _run_calls, _tiled, bq_inputs, ir_family, rs_bases)
 from test_gpu_chain import _add_ops, _inputs as chain_inputs, _op_index, _reference as chain_reference, _same, _spec as chain_spec
 from test_gpu_fir_full_wave import full_wave_channels
@@ -113,10 +113,10 @@ def test_resample_footprint(gpu_lib, C):
     counts, _ = rs_counts(RS_FI, RS_FO, sizes)
     tiles = {}
     for force in range(8):
-        tiles.setdefault(_expect_tile(C, force)[0], force)
+        tiles.setdefault(rs_expect_launch(C, force, 1, sms)["tile"], force)
     family = {}
     for tile, force in sorted(tiles.items()):
-        kernel = _expect_tile(C, force)[1]
+        kernel = rs_expect_launch(C, force, 1, sms)["kernel"]
         ch = _rs_chain(gpu_lib, RS_FI, RS_FO, C, RS_BW, force)
         want = _run_calls(ch, x, sizes)
         ch.close()
@@ -135,7 +135,7 @@ def test_resample_footprint(gpu_lib, C):
             for k, p in enumerate(plans):
                 if counts[k] == 0:
                     continue
-                warps = _expect_warps(C, counts[k], sms) if tile >= 4 else (2 if tile == 2 else 4)
+                warps = rs_expect_launch(C, force, counts[k], sms)["warps"]
                 assert (p["tile"], p["kernel"], p["warps"], p["out_align"]) == (tile, kernel, warps, 8 if layout[1] else 16), (C, layout, k, p)
             _same(got, want, "C%d tile %d %s vs host mode" % (C, tile, _layout_id(layout)))
 

@@ -37,8 +37,8 @@ import zlib
 import numpy as np
 import pytest
 
-from accuracy import (FIR_CASES, FIR_EDGES, RS_TILE_Q, dyadic_signal, env, fir_b0, fir_nan_window, rs_nan_windows)
-from test_gpu_accuracy import (BQ_CASCADE, BQ_SECTIONS, RS_SHAPES, _drain, _expect_tile, _ragged_sizes, _record,
+from accuracy import (FIR_CASES, FIR_EDGES, dyadic_signal, env, fir_b0, fir_nan_window, rs_expect_launch, rs_nan_windows)
+from test_gpu_accuracy import (BQ_CASCADE, BQ_SECTIONS, RS_SHAPES, _drain, _ragged_sizes, _record,
                                _run_calls, _rs_chain, ir_family, rs_bases, _tiled)
 
 pytestmark = pytest.mark.gpu
@@ -250,9 +250,10 @@ def _rs_poisons(sizes, C, in_len):
 
 def _rs_check(name, gpu_lib, fi, fo, bw, want, got, counts, poisons, tile):
     p = gpu_lib.resample_params(fi, fo, bw)
+    Q = rs_expect_launch(want.shape[1], tile, 1, 1)["Q"]   # output frames per CTA of the tile that ran
     _isolated(want, got, poisons, name)
     for k, n in poisons:
-        exact, near = rs_nan_windows(n, counts, p["n"], p["d"], p["in_len"], p["out_delay"], RS_TILE_Q[tile])
+        exact, near = rs_nan_windows(n, counts, p["n"], p["d"], p["in_len"], p["out_delay"], Q)
         diff = _differs(want[:, k], got[:, k])
         assert diff.any(), (name, k, n, "the sample never reached the output")
         bad = np.nonzero(diff & ~near)[0]
@@ -276,7 +277,7 @@ def _rs_case(gpu_lib, name, fi, fo, C, sizes, force=None, poll=None, bw=0.939, s
     poisons = _rs_poisons(sizes, C, gpu_lib.resample_params(fi, fo, bw)["in_len"])
     want, got, plan = _twice(lambda: _rs_chain(gpu_lib, fi, fo, C, bw, force), x, poisons, _rs_run(sizes, poll), fresh=not poll)
     tile = plan[0]["tile"]
-    assert tile == _expect_tile(C, force or 0)[0], (name, plan)
+    assert tile == rs_expect_launch(C, force or 0, 1, 1)["tile"], (name, plan)
     counts = [o.shape[0] for o in want]
     _rs_check(name, gpu_lib, fi, fo, bw, _cat(want, C), _cat(got, C), counts, poisons, tile)
     return plan[0]
@@ -297,7 +298,7 @@ def test_resample_variants_nonfinite(gpu_lib, shape):
     for C in RS_NF_SHAPES[shape]:
         seen = set()
         for force in range(8):
-            tile = _expect_tile(C, force)[0]
+            tile = rs_expect_launch(C, force, 1, 1)["tile"]
             if tile in seen:
                 continue
             seen.add(tile)

@@ -3,7 +3,7 @@ against brute-force numpy models that push a NaN through the same block structur
 import numpy as np
 import pytest
 
-from accuracy import RS_TILE_Q, fir_b0, fir_level_taps, fir_nan_window, rs_nan_windows
+from accuracy import fir_b0, fir_level_taps, fir_nan_window, rs_expect_launch, rs_nan_windows
 
 
 def _fir_model(N, n, taps, levels):
@@ -88,7 +88,7 @@ def _rs_model(counts, n_, d, in_len, out_delay, Q, G):
 
 
 @pytest.mark.parametrize("n_,d,in_len,delay", [(3, 4, 10, 2), (4, 3, 9, 5), (1, 6, 13, 0), (6, 1, 7, 3), (5, 7, 11, 1)])
-@pytest.mark.parametrize("Q", sorted(set(RS_TILE_Q.values())) + [8])
+@pytest.mark.parametrize("Q", sorted({rs_expect_launch(4, tile, 1, 1)["Q"] for tile in range(1, 8)}) + [8])
 def test_rs_nan_windows_against_a_tiled_model(n_, d, in_len, delay, Q):
     """Small rates, random non-zero taps, ragged calls (the drain is more calls): the tile mask equals the model's
     non-finite outputs for every input row n, and holds the exact window."""
