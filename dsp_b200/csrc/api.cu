@@ -9,6 +9,7 @@
 // concurrently.  There is no cross-shard data dependency, hence no collective.
 #include "common.cuh"
 #include "ops.h"
+#include "biquad_plan.h"
 #include "resample_plan.h"
 #include "fft.cuh"
 #include "../../include/dsp_b200.h"
@@ -589,9 +590,9 @@ int dspb200_chain_add_biquad(dspb200_chain *c, int n_stages, const double *coefs
 {
 	if (!c || !coefs || n_stages < 1) return -1;
 	const int C = c->channels;
-	// long cascades are cut into operators of <= 16 stages
-	for (int st0 = 0; st0 < n_stages; st0 += 16) {
-		const int ns = (n_stages - st0 < 16) ? n_stages - st0 : 16;
+	// long cascades are cut into operators of <= BQ_MAX_STAGES stages
+	for (int st0 = 0; st0 < n_stages; st0 += BQ_MAX_STAGES) {
+		const int ns = (n_stages - st0 < BQ_MAX_STAGES) ? n_stages - st0 : BQ_MAX_STAGES;
 		FOR_EACH_SHARD(c, s) {
 			CUDA_TRY(cudaSetDevice(s->device), return -1);
 			std::vector<double> slab((size_t) ns * s->ch_count * 5);

@@ -36,19 +36,9 @@
 // pairs; four channels per CTA halves the grid and loses more than it gains at 256 channels.)  Algorithmic bytes: 16 per sample.
 #include "common.cuh"
 #include "ops.h"
+#include "biquad_plan.h"
 
 namespace dspb200 {
-
-constexpr int BQ_L = 16;           // frames per lane
-constexpr int BQ_MAX_STAGES = 16;  // stages fused into one operator
-constexpr int BQ_NPOW = 6;         // M^(L 2^r), r = 0..5
-// per channel and stage: 5 coefficients (+1 pad), BQ_NPOW 2x2 matrices M^(L 2^r), the basis T and T^-1 (2x2 each), and
-// G[i] = T^-1 A^(L-1-i) B (2 x L), contiguous; every piece starts on a 16-byte boundary so that the kernel reads the
-// table with 128-bit shared loads
-constexpr double BQ_EPS_MIN = 1.0 / 32;
-constexpr int BQ_OFF_P = 6, BQ_OFF_T = BQ_OFF_P + 4 * BQ_NPOW, BQ_OFF_G = BQ_OFF_T + 8;
-constexpr int BQ_TBL = BQ_OFF_G + 2 * BQ_L;
-static_assert(BQ_TBL % 2 == 0 && BQ_OFF_G % 2 == 0, "table pieces must stay 16-byte aligned");
 
 struct M2 { double a, b, c, d; };  // [[a, b], [c, d]]
 
@@ -56,25 +46,6 @@ __device__ __forceinline__ double2 m2_apply(const M2 &m, double2 v)
 {
 	return make_double2(fma(m.a, v.x, m.b * v.y), fma(m.c, v.x, m.d * v.y));
 }
-
-// CH adjacent channels share a CTA; a warp's lanes are (32 / CH consecutive chunks) x (CH channels), channel
-// fastest, so that one load instruction touches 32 / CH rows and uses CH x 8 contiguous bytes of each.
-// SPLIT: two CTAs per channel pair, each on one half (2048 frames) of a 4096-frame tile, 8 warps each -- two of
-// them fit an SM, so that one CTA's barriers, table loads and block I/O hide behind the other's arithmetic.  The
-// second half needs, per stage, the state the first half ends in: the first half publishes it (state, fence, flag)
-// as soon as its stage is done and the second half picks it up right before that stage's carry step, i.e. it runs
-// one stage behind (decoupled look-back along time; CTAs of the first half have the lower block indices, so they
-// are always scheduled before the CTAs that wait for them).
-template <int CH, bool SPLIT = false>
-struct BqCfg {
-	static_assert(CH == 1 || CH == 2 || CH == 4, "1, 2 or 4 channels per CTA");
-	static_assert(!SPLIT || CH == 2, "the split form is built for channel pairs");
-	static constexpr int CPW = 32 / CH;                         // chunks per warp
-	static constexpr int LOGW = (CH == 1) ? 5 : (CH == 2) ? 4 : 3;
-	static constexpr int WARPS = SPLIT ? 8 : (CH == 1) ? 8 : 16;
-	static constexpr int THREADS = 32 * WARPS;
-	static constexpr long TILE = (long) BQ_L * CPW * WARPS;     // frames per tile
-};
 
 struct BqSplitArgs {
 	double *xstate;   // [C][S][2]: state at the end of the first half, per stage
@@ -216,27 +187,6 @@ __global__ void __launch_bounds__(BqCfg<CH, SPLIT>::THREADS, SPLIT ? 2 : 1) k_bq
 	}
 }
 
-template <int CH>
-static int bq_launch(const double *in, double *out, const double *tbl, double *zstate, int C, int S, long frames, cudaStream_t st)
-{
-	LAUNCH((k_bq_cascade<CH>), (C + CH - 1) / CH, BqCfg<CH>::THREADS, (size_t) CH * S * BQ_TBL * sizeof(double), st, in, out, tbl, zstate, C, S, frames, BqSplitArgs{});
-	return 0;
-}
-
-// split form: one launch per 4096 frames, two CTAs per channel pair
-static int bq_launch_split(const double *in, double *out, const double *tbl, double *zstate, int C, int S, long frames, cudaStream_t st, BqSplitArgs sp, int *epoch)
-{
-	using Cfg = BqCfg<2, true>;
-	const long span = 2 * Cfg::TILE;
-	for (long base = 0; base < frames; base += span) {
-		const long n = (frames - base < span) ? frames - base : span;
-		sp.epoch = ++*epoch;
-		LAUNCH((k_bq_cascade<2, true>), dim3((C + 1) / 2, 2), Cfg::THREADS, (size_t) 2 * S * BQ_TBL * sizeof(double), st, in + base * C, out + base * C, tbl,
-		       zstate, C, S, n, sp);
-	}
-	return 0;
-}
-
 struct BiquadOp : Op {
 	int S = 0;
 	std::vector<double> h_coefs;   // [S][C][5] as handed in (kept so neighbouring cascades can be fused)
@@ -244,12 +194,13 @@ struct BiquadOp : Op {
 	double *d_xstate = nullptr;   // split form: per-stage state between the two halves of a tile
 	int *d_flag = nullptr;
 	int epoch = 0;
+	BqLaunch last;   // the last call's launches (describe(): ch = 0 before the first call)
 
 	const char *name() const override { return "biquad"; }
 	std::string describe() const override
 	{
 		char buf[96];
-		snprintf(buf, sizeof(buf), "{\"op\":\"biquad\",\"stages\":%d}", S);
+		snprintf(buf, sizeof(buf), "{\"op\":\"biquad\",\"stages\":%d,\"ch\":%d,\"split\":%d}", S, last.ch, last.split);
 		return buf;
 	}
 	~BiquadOp() override { dev_free(d_tbl); dev_free(d_zstate); dev_free(d_xstate); dev_free(d_flag); }
@@ -263,26 +214,16 @@ struct BiquadOp : Op {
 	{
 		if (frames <= 0) return 0;
 		ProfScope prof("biquad", st);
-		// channels per CTA: wider rows per load as long as the grid still covers the SMs
-		static const int force = getenv("DSP_B200_BQ_CH") ? atoi(getenv("DSP_B200_BQ_CH")) : 0;
-		// Always channel pairs: the scan's association order depends on the chunks per warp, and a channel's
-		// result must not depend on how the chain was sharded (tests: sharded == unsharded, bit for bit).
-		const int chp = force ? force : 2;
-		// Split form (two 8-warp CTAs per channel pair with a per-stage look-back of the first half's state): slower
-		// than one 16-warp CTA on full tiles (the second half trails by a stage and the two CTAs of a pair contend for
-		// the same SM's FP64 pipe instead of hiding each other) -- but calls of at most 2048 frames have no second
-		// half, and 8 warps on such a block beat 16 half-idle ones.  DSP_B200_BQ_SPLIT=1 forces it everywhere, =0 nowhere.
-		static const int split_env = getenv("DSP_B200_BQ_SPLIT") ? atoi(getenv("DSP_B200_BQ_SPLIT")) : -1;
-		const bool split = (split_env >= 0) ? split_env != 0 : frames <= BqCfg<2, true>::TILE;
-		int rc;
-		if (chp == 2 && split) {
-			BqSplitArgs sp = { d_xstate, d_flag, 0 };
-			rc = bq_launch_split(in, out, d_tbl, d_zstate, channels, S, frames, st, sp, &epoch);
+		static const int force_ch = getenv("DSP_B200_BQ_CH") ? atoi(getenv("DSP_B200_BQ_CH")) : 0;
+		static const int force_split = getenv("DSP_B200_BQ_SPLIT") ? atoi(getenv("DSP_B200_BQ_SPLIT")) : -1;
+		last = bq_launch(channels, S, frames, force_ch, force_split);
+		const auto k_bq = last.split ? k_bq_cascade<2, true> : (last.ch == 4) ? k_bq_cascade<4> : (last.ch == 2) ? k_bq_cascade<2> : k_bq_cascade<1>;
+		for (long i = 0, base = 0; i < last.launches; ++i, base += last.span) {
+			const BqSplitArgs sp = last.split ? BqSplitArgs{ d_xstate, d_flag, ++epoch } : BqSplitArgs{};
+			LAUNCH(k_bq, dim3(last.grid, 1 + last.split), last.threads, last.smem, st, in + base * channels, out + base * channels, d_tbl, d_zstate,
+			       channels, S, (frames - base < last.span) ? frames - base : last.span, sp);
 		}
-		else if (chp == 4) rc = bq_launch<4>(in, out, d_tbl, d_zstate, channels, S, frames, st);
-		else if (chp == 2) rc = bq_launch<2>(in, out, d_tbl, d_zstate, channels, S, frames, st);
-		else rc = bq_launch<1>(in, out, d_tbl, d_zstate, channels, S, frames, st);
-		return rc ? -1 : frames;
+		return frames;
 	}
 };
 
@@ -297,49 +238,7 @@ Op *make_biquad_op(int slab_channels, int fs, int n_stages, const double *coefs)
 	op->channels = C; op->fs_in = op->fs_out = fs; op->S = S;
 	op->h_coefs.assign(coefs, coefs + (size_t) S * C * 5);
 
-	// coefs arrive as [stage][channel][5]; the kernel wants one contiguous table per channel (a CTA reads one channel)
-	std::vector<double> tbl((size_t) C * S * BQ_TBL);
-	for (int c = 0; c < C; ++c) {
-		for (int st = 0; st < S; ++st) {
-			const double *cf = &coefs[((size_t) st * C + c) * 5];
-			double *t = &tbl[((size_t) c * S + st) * BQ_TBL];
-			for (int k = 0; k < 5; ++k) t[k] = cf[k];
-			// A = [[-c3, 1], [-c4, 0]], B = (c1 - c3 c0, c2 - c4 c0): z' = A z + B s   (biquad.h:79-81 with r = c0 s + m0)
-			const long double Az[4] = { -(long double) cf[3], 1.0L, -(long double) cf[4], 0.0L };
-			const long double Bz[2] = { (long double) cf[1] - (long double) cf[3] * cf[0], (long double) cf[2] - (long double) cf[4] * cf[0] };
-			// the scan's basis (header): z = T w, w' = M w + T^-1 B s
-			const long double al = -(long double) cf[3] / 2, d2 = al * al - (long double) cf[4];
-			long double eps = sqrtl(fabsl(d2));
-			if (eps < BQ_EPS_MIN) eps = BQ_EPS_MIN;
-			const long double T[4] = { 1.0L, 0.0L, -al, eps }, Ti[4] = { 1.0L, 0.0L, al / eps, 1.0L / eps };
-			const long double AT[4] = { Az[0] * T[0] + Az[1] * T[2], Az[0] * T[1] + Az[1] * T[3], Az[2] * T[0] + Az[3] * T[2], Az[2] * T[1] + Az[3] * T[3] };
-			const long double A[4] = { Ti[0] * AT[0] + Ti[1] * AT[2], Ti[0] * AT[1] + Ti[1] * AT[3], Ti[2] * AT[0] + Ti[3] * AT[2], Ti[2] * AT[1] + Ti[3] * AT[3] };
-			const long double Bv[2] = { Ti[0] * Bz[0] + Ti[1] * Bz[1], Ti[2] * Bz[0] + Ti[3] * Bz[1] };
-			for (int k = 0; k < 4; ++k) {
-				t[BQ_OFF_T + k] = (double) T[k];
-				t[BQ_OFF_T + 4 + k] = (double) Ti[k];
-			}
-			// G[i] = M^(L-1-i) T^-1 B, i = L-1 .. 0, and M^L on the way
-			long double g[2] = { Bv[0], Bv[1] };
-			for (int i = BQ_L - 1; i >= 0; --i) {
-				t[BQ_OFF_G + 2 * i] = (double) g[0];
-				t[BQ_OFF_G + 2 * i + 1] = (double) g[1];
-				const long double n0 = A[0] * g[0] + A[1] * g[1], n1 = A[2] * g[0] + A[3] * g[1];
-				g[0] = n0; g[1] = n1;
-			}
-			long double a[4] = { 1.0L, 0.0L, 0.0L, 1.0L };
-			for (int i = 0; i < BQ_L; ++i) {
-				const long double u[4] = { A[0] * a[0] + A[1] * a[2], A[0] * a[1] + A[1] * a[3], A[2] * a[0] + A[3] * a[2], A[2] * a[1] + A[3] * a[3] };
-				for (int k = 0; k < 4; ++k) a[k] = u[k];
-			}
-			// M^(L 2^r) by repeated squaring
-			for (int r = 0; r < BQ_NPOW; ++r) {
-				for (int k = 0; k < 4; ++k) t[BQ_OFF_P + 4 * r + k] = (double) a[k];
-				const long double u[4] = { a[0] * a[0] + a[1] * a[2], a[0] * a[1] + a[1] * a[3], a[2] * a[0] + a[3] * a[2], a[2] * a[1] + a[3] * a[3] };
-				for (int k = 0; k < 4; ++k) a[k] = u[k];
-			}
-		}
-	}
+	const std::vector<double> tbl = bq_table(C, S, coefs);
 	op->d_tbl = dev_alloc<double>(tbl.size(), false);
 	op->d_zstate = dev_alloc<double>((size_t) C * S * 2, true);
 	op->d_xstate = dev_alloc<double>((size_t) C * S * 2, true);

@@ -7,7 +7,8 @@ about 23 + log2(taps) bits: at 131072 taps and beyond it is still far inside the
 FP64 FFT convolution of the integer numerators is then within a small fraction of a unit of the exact
 integers, and rounding to the grid recovers them exactly.
 
-Biquad: `biquad_truth` runs the same double coefficients through scipy's lfilter in 80-bit long double.
+Biquad: `biquad_truth` runs the same double coefficients through scipy's lfilter in 80-bit long double;
+`bq_expect_launch` restates the kernel form each call gets.
 
 Resample: `resample_taps_truth` is the tap table G of the polyphase form (resample.cu header) in long double, built
 from the reference's own sinc samples; `resample_truth` evaluates the emitted stream from it in long double, and
@@ -123,6 +124,23 @@ def biquad_truth(x, coefs):
             k = coefs[st, c].astype(np.longdouble)
             y[:, c] = lfilter(k[:3], np.array([1.0, k[3], k[4]], dtype=np.longdouble), y[:, c])
     return y
+
+
+BQ_TBL = 70   # doubles per channel and stage: 5 coefficients and a pad, 6 matrices M^(16 2^r), T, T^-1, G (2 x 16)
+
+
+def bq_expect_launch(C, S, frames, force_ch=None, force_split=None):
+    """The launch of a biquad call of `frames` frames on C channels and S stages, with DSP_B200_BQ_CH=`force_ch` and
+    DSP_B200_BQ_SPLIT=`force_split` (None: unset) -- bq_launch() of dsp_b200/csrc/biquad_plan.h, restated.  Two
+    channels per CTA unless the knob asks for 4, or for anything but 0, 2 and 4, which runs one.  The split form (two
+    8-warp CTAs per channel pair, one launch per 4096 frames) runs on pairs only: on calls of at most 2048 frames, or as
+    a non-negative DSP_B200_BQ_SPLIT says (0: never, else always).  The others take 16 warps (8 on one channel per
+    CTA) and one launch.  smem: the CTA's channel tables."""
+    ch = 2 if force_ch in (None, 0, 2) else 4 if force_ch == 4 else 1
+    split = ch == 2 and (frames <= 2048 if force_split is None or force_split < 0 else force_split != 0)
+    span = 4096 if split else frames
+    return dict(ch=ch, split=int(split), threads=32 * (8 if split or ch == 1 else 16), grid=-(-C // ch),
+                smem=ch * S * BQ_TBL * 8, span=span, launches=-(-frames // span))
 
 
 def biquad_err(got, truth):
@@ -312,8 +330,8 @@ CSRC = os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file__))),
 
 
 def header_lib(tmp_dir, name, source):
-    """Compile a C++ driver of a host-only header of dsp_b200/csrc (fir_plan.h, resample_plan.h) with g++ alone (no
-    CUDA); -> ctypes.CDLL."""
+    """Compile a C++ driver of a host-only header of dsp_b200/csrc (fir_plan.h, resample_plan.h, biquad_plan.h) with
+    g++ alone (no CUDA); -> ctypes.CDLL."""
     src, so = tmp_dir / (name + ".cpp"), tmp_dir / ("lib%s.so" % name)
     src.write_text(source)
     subprocess.run(["g++", "-std=c++17", "-O1", "-Wall", "-Werror", "-shared", "-fPIC", "-I", CSRC, str(src), "-o", str(so)], check=True)

@@ -36,8 +36,8 @@ import zlib
 import numpy as np
 import pytest
 
-from accuracy import (F2, F4, FIR_CASES, FIR_EDGES, H_MAX, RS_RATIOS, RsPacing, _fir_plan, _ladder, biquad_within_ref, dyadic_signal,
-                      dyadic_taps, env, exact_conv, fir_nerr, resample_taps_truth, resample_truth, rs_counts, rs_expect_launch, rs_nerr,
+from accuracy import (F2, F4, FIR_CASES, FIR_EDGES, H_MAX, RS_RATIOS, RsPacing, _fir_plan, _ladder, biquad_within_ref, bq_expect_launch,
+                      dyadic_signal, dyadic_taps, env, exact_conv, fir_nerr, resample_taps_truth, resample_truth, rs_counts, rs_expect_launch, rs_nerr,
                       taps_norm)
 
 pytestmark = pytest.mark.gpu
@@ -396,9 +396,10 @@ def _design(gpu_lib, sec):
 @pytest.mark.parametrize("name", list(BQ_SECTIONS))
 def test_biquad_ill_conditioned_sections(gpu_lib, name, form):
     """One section, four slow, large inputs; calls of 2048 frames (split form) or 4096 (16-warp form), ragged calls
-    after a reset.  Measured (H100 80GB HBM3, 400 W): err_gpu at most 0.25 of its bound in every case.  The 10 Hz /
-    192 kHz lowpass with Q 5 is at most 2.9e-12 relative over its inputs (the FP64 recurrence: up to 1.6e-10); with
-    the scan in the companion basis (before biquad.cu's basis change) it was 1.4e-9 on the sine input."""
+    after a reset.  describe() shows that every call of F frames ran the form named, and every call the form
+    bq_expect_launch gives.  Measured (H100 80GB HBM3, 400 W): err_gpu at most 0.25 of its bound in every case.  The
+    10 Hz / 192 kHz lowpass with Q 5 is at most 2.9e-12 relative over its inputs (the FP64 recurrence: up to 1.6e-10);
+    with the scan in the companion basis (before biquad.cu's basis change) it was 1.4e-9 on the sine input."""
     sec = BQ_SECTIONS[name]
     fs = sec[1]
     coefs = _design(gpu_lib, sec)[None, :]
@@ -406,11 +407,18 @@ def test_biquad_ill_conditioned_sections(gpu_lib, name, form):
     x = bq_inputs(fs, N, seed=len(name))
     F = 2048 if form == "split" else 4096
     ch = gpu_lib.Chain(fs, 4).add_biquad(coefs)
-    got = np.concatenate([ch.run(x[i:i + F]).copy() for i in range(0, N, F)])
+
+    def run(a, b):
+        y = ch.run(x[a:b]).copy()
+        d, want = ch.describe()[0], bq_expect_launch(4, 1, b - a)
+        assert (d["ch"], d["split"]) == (want["ch"], want["split"]), (a, b, d)
+        assert b - a != F or d["split"] == (form == "split"), (a, b, d)
+        return y
+    got = np.concatenate([run(i, min(i + F, N)) for i in range(0, N, F)])
     bq_check("%s/%s" % (name, form), got, x, coefs)
     ch.reset()
     cuts = [0, 1, 2047, 2049, 4096, 8192, 8193, 12287, 16384, N] if form == "split" else [0, 4095, 8191, 8192, 12289, 20000, N]
-    got2 = np.concatenate([ch.run(x[a:b]).copy() for a, b in zip(cuts[:-1], cuts[1:])])
+    got2 = np.concatenate([run(a, b) for a, b in zip(cuts[:-1], cuts[1:])])
     bq_check("%s/%s/ragged" % (name, form), got2, x, coefs)
     ch.close()
 

@@ -37,7 +37,8 @@ import zlib
 import numpy as np
 import pytest
 
-from accuracy import (FIR_CASES, FIR_EDGES, dyadic_signal, env, fir_b0, fir_nan_window, rs_expect_launch, rs_nan_windows)
+from accuracy import (FIR_CASES, FIR_EDGES, bq_expect_launch, dyadic_signal, env, fir_b0, fir_nan_window, rs_expect_launch,
+                      rs_nan_windows)
 from test_gpu_accuracy import (BQ_CASCADE, BQ_SECTIONS, RS_SHAPES, _drain, _ragged_sizes, _record,
                                _run_calls, _rs_chain, ir_family, rs_bases, _tiled)
 
@@ -379,7 +380,11 @@ def bq_case(gpu_lib, name, stages, C, sizes, identity=False, absorb=False):
         b.close()
         assert a.n_ops == 1
         return a
-    want, got, _ = _twice(make, x, poisons, _calls(sizes))
+    want, got, plan = _twice(make, x, poisons, _calls(sizes))
+    # the form of the last call, under the knobs the library read from this process's environment
+    knob = lambda v: int(os.environ[v]) if v in os.environ else None
+    form = bq_expect_launch(C, stages, sizes[-1], knob("DSP_B200_BQ_CH"), knob("DSP_B200_BQ_SPLIT"))
+    assert (plan[0]["ch"], plan[0]["split"]) == (form["ch"], form["split"]), (name, plan)
     want, got = _cat(want, C), _cat(got, C)
     _isolated(want, got, poisons, name)
     ks = [k for k, _ in poisons]
