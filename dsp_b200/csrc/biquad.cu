@@ -28,7 +28,8 @@
 // [[alpha, eps], [+-eps, alpha]]: symmetric for real poles, a scaled rotation for complex ones, normal either way, so
 // the powers M^k stay bounded by 1 and the scan keeps the precision of its inputs.  eps is clamped below at 1/32 for
 // (near-)double poles, where T would be singular; M is then only mildly non-normal.  Measured on the 10 Hz / 192 kHz
-// sections the GPU lands within a few times the FP64 recurrence's error (tests/test_gpu_accuracy.py).
+// sections the GPU lands within a few times the FP64 recurrence's error (tests/test_gpu_accuracy.py), on sections near
+// Nyquist (poles near z = -1) at about that error (tests/test_gpu_dropin_effects.py; see step (1) below).
 // A stage that does not act on a channel carries the identity section {1,0,0,0,0}.
 // Global accesses: one load instruction of a warp touches 16 rows (frames) and uses 16 contiguous bytes of
 // each -- half of every 32-byte sector, the neighbouring CTA uses the other half at about the same time, so
@@ -103,16 +104,20 @@ __global__ void __launch_bounds__(BqCfg<CH, SPLIT>::THREADS, SPLIT ? 2 : 1) k_bq
 				P[r] = M2{ lo.x, lo.y, hi.x, hi.y };
 			}
 			// (1) zero-state end state of a FULL chunk as a dot product (a partial last chunk is nobody's predecessor:
-			//     its value is never used; missing samples are zeros)
+			//     its value is never used; missing samples are zeros).  Two accumulators for ILP, each over consecutive
+			//     frames (the first and the second half of the chunk): near Nyquist G alternates in sign, and splitting
+			//     the terms into even and odd frames would build two large sums that cancel at the end -- 4 to 8 times
+			//     the FP64 recurrence's error on a smooth input (tests/test_gpu_dropin_effects.py); in order, the
+			//     partial sums stay as small as the terms.
 			const double2 *G = t + BQ_OFF_G / 2;
 			double ex0 = 0.0, ex1 = 0.0, ey0 = 0.0, ey1 = 0.0;
 #pragma unroll
-			for (int i = 0; i < BQ_L; i += 2) {
-				const double2 g0 = G[i], g1 = G[i + 1];
+			for (int i = 0; i < BQ_L / 2; ++i) {
+				const double2 g0 = G[i], g1 = G[i + BQ_L / 2];
 				ex0 = fma(g0.x, y[i], ex0);
 				ey0 = fma(g0.y, y[i], ey0);
-				ex1 = fma(g1.x, y[i + 1], ex1);
-				ey1 = fma(g1.y, y[i + 1], ey1);
+				ex1 = fma(g1.x, y[i + BQ_L / 2], ex1);
+				ey1 = fma(g1.y, y[i + BQ_L / 2], ey1);
 			}
 			// (2) inclusive scan over the chunks of this warp (uniform matrix A^L per chunk); lanes CH apart
 			double2 sc = make_double2(ex0 + ex1, ey0 + ey1);
@@ -194,6 +199,7 @@ struct BiquadOp : Op {
 	double *d_xstate = nullptr;   // split form: per-stage state between the two halves of a tile
 	int *d_flag = nullptr;
 	int epoch = 0;
+	bool ran = false;   // d_zstate may hold state: run() since construction or the last reset()
 	BqLaunch last;   // the last call's launches (describe(): ch = 0 before the first call)
 
 	const char *name() const override { return "biquad"; }
@@ -208,11 +214,13 @@ struct BiquadOp : Op {
 	void reset(cudaStream_t st) override
 	{
 		cudaMemsetAsync(d_zstate, 0, (size_t) channels * S * 2 * sizeof(double), st);
+		ran = false;
 	}
 
 	long run(long frames, const double *in, double *out, cudaStream_t st) override
 	{
 		if (frames <= 0) return 0;
+		ran = true;
 		ProfScope prof("biquad", st);
 		static const int force_ch = getenv("DSP_B200_BQ_CH") ? atoi(getenv("DSP_B200_BQ_CH")) : 0;
 		static const int force_split = getenv("DSP_B200_BQ_SPLIT") ? atoi(getenv("DSP_B200_BQ_SPLIT")) : -1;
@@ -248,12 +256,12 @@ Op *make_biquad_op(int slab_channels, int fs, int n_stages, const double *coefs)
 	return op.release();
 }
 
-// Two adjacent cascades over the same slab become one operator (one pass over the block).
-// Only legal before the first run()/after reset.
+// Two adjacent cascades over the same slab become one operator (one pass over the block).  The fused
+// operator starts from zero state, so cascades that have run since their last reset() are not fused.
 Op *fuse_biquad_ops(Op *a, Op *b)
 {
 	BiquadOp *x = dynamic_cast<BiquadOp *>(a), *y = dynamic_cast<BiquadOp *>(b);
-	if (!x || !y || x->channels != y->channels || x->fs_in != y->fs_in || x->S + y->S > BQ_MAX_STAGES) return nullptr;
+	if (!x || !y || x->ran || y->ran || x->channels != y->channels || x->fs_in != y->fs_in || x->S + y->S > BQ_MAX_STAGES) return nullptr;
 	std::vector<double> all(x->h_coefs);
 	all.insert(all.end(), y->h_coefs.begin(), y->h_coefs.end());
 	return make_biquad_op(x->channels, x->fs_in, x->S + y->S, all.data());

@@ -8,7 +8,8 @@ namespace dspb200 {
 Op *make_gain_op(int slab_channels, int fs, const double *mult, const double *add);
 // biquad.c:296-315; coefs[stage][slab_channels][5]
 Op *make_biquad_op(int slab_channels, int fs, int n_stages, const double *coefs);
-// returns a new operator equivalent to a followed by b, or nullptr if they cannot be fused
+// returns a new operator equivalent to a followed by b, or nullptr if they cannot be fused (either has run
+// since its last reset)
 Op *fuse_biquad_ops(Op *a, Op *b);
 // fir.c / fir_p.c; taps[filter_frames][filter_channels]; taps_cols[k] = filter column of the
 // k-th selected channel of this slab (ignored when filter_channels == 1)

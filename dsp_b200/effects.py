@@ -15,6 +15,7 @@ code that is NOT part of the accelerated path and stays the reference's C in a r
 import importlib
 import math
 import os
+import re
 
 import numpy as np
 
@@ -37,34 +38,63 @@ class ChainSyntaxError(ValueError):
     pass
 
 
-def parse_freq(s):
-    """util.c:49-63"""
+# what strtod() reads: leading white space, a sign, then a decimal number with an optional exponent, a hexadecimal
+# one with an optional binary exponent, inf[inity] or nan[(chars)] (no digit separators, unlike Python's float())
+_STRTOD = re.compile(r"\s*([+-]?)(?:(?P<dec>(?:[0-9]+\.?[0-9]*|\.[0-9]+)(?:[eE][+-]?[0-9]+)?)"
+                     r"|(?P<hex>0[xX](?:[0-9a-fA-F]+\.?[0-9a-fA-F]*|\.[0-9a-fA-F]+)(?:[pP][+-]?[0-9]+)?)"
+                     r"|(?P<inf>[iI][nN][fF](?:[iI][nN][iI][tT][yY])?)|(?P<nan>[nN][aA][nN](?:\([0-9A-Za-z_]*\))?))")
+
+
+def parse_num(s, what="value"):
+    """strtod() over the whole word, as the reference's CHECK_ENDPTR demands (util.c:35-47)."""
+    m = _STRTOD.fullmatch(s)
+    if not m:
+        raise ChainSyntaxError("failed to parse %s: %s" % (what, s))
+    sign = -1.0 if m.group(1) == "-" else 1.0
+    if m.group("dec"):
+        return sign * float(m.group("dec"))
+    if m.group("hex"):
+        h = m.group("hex")
+        return sign * float.fromhex(h if "p" in h.lower() else h + "p0")
+    return sign * float("inf" if m.group("inf") else "nan")
+
+
+def parse_int(s, what="value"):
+    """strtol(s, 10) over the whole word."""
+    if not re.fullmatch(r"\s*[+-]?[0-9]+", s):
+        raise ChainSyntaxError("failed to parse %s: %s" % (what, s))
+    return int(s)
+
+
+def parse_freq(s, what="f0"):
+    """util.c:49-63: a number, optionally followed by k"""
     if s.endswith("k"):
-        return float(s[:-1]) * 1000.0
-    return float(s)
+        return parse_num(s[:-1], what) * 1000.0
+    return parse_num(s, what)
 
 
 def parse_width(s):
     """biquad.c:27-89 -> (width, width_type)"""
     if s.startswith("bw") and len(s) > 2:
-        body = s[2:]
-        order, _, idx = body.partition(".")
-        order = int(order)
+        m = re.fullmatch(r"(\s*[+-]?[0-9]+)(?:\.(\s*[+-]?[0-9]+))?", s[2:])
+        if not m:
+            raise ChainSyntaxError("failed to parse width: %s" % s)
+        order = int(m.group(1))
         if order < 2:
             raise ChainSyntaxError("filter order must be >= 2")
         n_biquads = order // 2
-        p_idx = int(idx) if idx else 0
+        p_idx = int(m.group(2)) if m.group(2) is not None else 0
         if p_idx < 0 or p_idx >= n_biquads:
             raise ChainSyntaxError("filter index out of range")
         p_idx = n_biquads - p_idx
         return 1.0 / (2.0 * math.sin(math.pi / order * (p_idx - 0.5))), WIDTH_Q
     suffix = {"q": WIDTH_Q, "s": WIDTH_SLOPE, "d": WIDTH_SLOPE_DB, "o": WIDTH_BW_OCT, "h": WIDTH_BW_HZ, "k": WIDTH_BW_HZ}
     if s and s[-1] in suffix:
-        w = float(s[:-1])
+        w = parse_num(s[:-1], "width")
         if s[-1] == "k":
             w *= 1000.0
         return w, suffix[s[-1]]
-    return float(s), WIDTH_Q
+    return parse_num(s, "width"), WIDTH_Q
 
 
 def parse_selector(s, n):
@@ -169,7 +199,7 @@ class EffectsChain:
         if name in ("gain", "mult", "add"):
             if len(args) != 1:
                 raise ChainSyntaxError("%s: usage: %s value" % (name, name))
-            v = float(args[0])
+            v = parse_num(args[0], name)
             if name == "gain":
                 v = 10.0 ** (v / 20.0)
             if name == "add":
@@ -183,32 +213,53 @@ class EffectsChain:
         elif name == "hilbert":
             conv, do_align, angle = "fir", False, -math.pi / 2
             a = list(args)
-            while a and a[0].startswith("-") and not a[0][1:2].isdigit():
+            # dsp_getopt(argc - 1, "pzca:") (hilbert.c:36-54): options only in front of the last word
+            while len(a) > 1 and a[0].startswith("-") and len(a[0]) > 1:
                 o = a.pop(0)
-                for ch in o[1:]:
+                for i, ch in enumerate(o[1:]):
                     if ch == "p" or ch == "z":
                         conv = "fir_p"
                     elif ch == "c":
                         do_align = True
                     elif ch == "a":
-                        angle = float(a.pop(0)) / 180.0 * math.pi
+                        if o[i + 2:]:
+                            v = o[i + 2:]
+                        elif len(a) > 1:
+                            v = a.pop(0)
+                        else:
+                            raise ChainSyntaxError("hilbert: option -a needs an angle")
+                        angle = parse_num(v, "angle") / 180.0 * math.pi
+                        break
+                    else:
+                        raise ChainSyntaxError("hilbert: unknown option -%s" % ch)
             if len(a) != 1:
                 raise ChainSyntaxError("hilbert: usage: hilbert [-p|-z] [-c] [-a angle] taps")
+            n_taps = parse_int(a[0], "taps")
+            if n_taps <= 3 or n_taps % 2 == 0:
+                raise ChainSyntaxError("hilbert: taps must be > 3 and odd")
             if do_align:
                 raise NotImplementedError("hilbert -c needs the reference's align pass (C shim)")
-            taps = _lib.hilbert_taps(int(a[0]), angle)
+            taps = _lib.hilbert_taps(n_taps, angle)
             self._add_fir(conv, taps[:, None], sel)
         elif name == "resample":
             if len(args) not in (1, 2):
                 raise ChainSyntaxError("resample: usage: resample [bandwidth] fs")
-            bw = float(args[0]) if len(args) == 2 else 0.0
+            bw = parse_num(args[0], "bandwidth") if len(args) == 2 else 0.0
+            if len(args) == 2 and not 0.7 <= bw <= 0.999:
+                raise ChainSyntaxError("resample: bandwidth out of range: %s" % args[0])
             r = args[-1]
             if r.startswith("x"):
-                rate = self._fs * int(r[1:])
+                rate = self._fs * parse_int(r[1:], "fs multiplier")
             elif r.startswith("/"):
-                rate = self._fs // int(r[1:])
+                div = parse_int(r[1:], "fs divisor")
+                if div == 0 or self._fs % div:
+                    raise ChainSyntaxError("resample: %d is not a factor of %d" % (div, self._fs))
+                rate = self._fs // div
             else:
-                rate = int(round(parse_freq(r)))
+                f = parse_freq(r, "fs")
+                rate = int(math.floor(abs(f) + 0.5)) * (1 if f >= 0 else -1)    # lround()
+            if rate <= 0:
+                raise ChainSyntaxError("resample: rate out of range: %s" % r)
             if self._align_discard:
                 raise NotImplementedError("fir latency followed by a rate change needs the reference's align pass")
             if rate != self._fs:
@@ -238,10 +289,16 @@ class EffectsChain:
 
     def _design(self, name, args):
         fs = self._fs
+        if args and args[0].startswith("-r"):
+            raise NotImplementedError("biquad -r (reverse IIR) is designed by the reference (C shim)")
         if name == "biquad":
-            b0, b1, b2, a0, a1, a2 = (float(v) for v in args)
+            if len(args) != 6:
+                raise ChainSyntaxError("biquad: expected 6 arguments")
+            b0, b1, b2, a0, a1, a2 = (parse_num(v, "coefficient") for v in args)
             return (b0 / a0, b1 / a0, b2 / a0, a1 / a0, a2 / a0)
         if name == "deemph":
+            if args:
+                raise ChainSyntaxError("deemph: expected no arguments")
             preset = {44100: (5283, 0.4845, -9.477), 48000: (5356, 0.479, -9.62)}.get(fs)
             if not preset:
                 raise ChainSyntaxError("deemph: sample rate must be 44100 or 48000")
@@ -253,12 +310,22 @@ class EffectsChain:
         vals = []
         for kind, a in zip(sig, args):
             if kind == "f":
-                vals.append(parse_freq(a))
+                f = parse_freq(a)
+                if not 0.0 <= f < fs / 2.0:       # CHECK_FREQ (util.h:36-37)
+                    raise ChainSyntaxError("%s: frequency out of range: %s" % (name, a))
+                vals.append(f)
             elif kind == "w":
                 w, wt = parse_width(a)
+                if not w > 0.0:
+                    raise ChainSyntaxError("%s: width out of range: %s" % (name, a))
+                # biquad.c:476,484,492,495: slope widths only on the shelves, only Q on the transforms
+                if wt in (WIDTH_SLOPE, WIDTH_SLOPE_DB) and name not in ("lowshelf", "highshelf"):
+                    raise ChainSyntaxError("%s: invalid width type: %s" % (name, a))
+                if sig == "fwfw" and wt != WIDTH_Q:
+                    raise ChainSyntaxError("%s: invalid width type: %s" % (name, a))
                 vals.append(w)
             else:
-                vals.append(float(a))
+                vals.append(parse_num(a, "gain"))
         if sig == "f":
             arg = (vals[0], 0.0, 0.0, 0.0)
         elif sig == "fg":
@@ -340,17 +407,21 @@ def build_chain(chain_str, fs, channels, dir=None, devices=None, slabs_per_devic
     words = chain_str.split()
     known = set(BIQUAD_TYPES) | {"biquad", "deemph", "gain", "mult", "add", "fir", "fir_p", "hilbert", "resample"}
     i = 0
-    while i < len(words):
-        w = words[i]
-        if w.startswith(":"):
-            sel = parse_selector(w[1:], channels)
-            i += 1
-            continue
-        if w not in known:
-            raise ChainSyntaxError("unknown or unaccelerated effect: %r" % w)
-        j = i + 1
-        while j < len(words) and not words[j].startswith(":") and words[j] not in known:
-            j += 1
-        ec.add_effect(w, words[i + 1:j], sel, dir)
-        i = j
-    return ec.finish()
+    try:
+        while i < len(words):
+            w = words[i]
+            if w.startswith(":"):
+                sel = parse_selector(w[1:], channels)
+                i += 1
+                continue
+            if w not in known:
+                raise ChainSyntaxError("unknown or unaccelerated effect: %r" % w)
+            j = i + 1
+            while j < len(words) and not words[j].startswith(":") and words[j] not in known:
+                j += 1
+            ec.add_effect(w, words[i + 1:j], sel, dir)
+            i = j
+        return ec.finish()
+    except BaseException:
+        ec.close()          # a refused chain frees its device chain now, not when the collector finds it
+        raise

@@ -149,13 +149,16 @@ def biquad_err(got, truth):
     return float(np.sqrt(np.mean(d * d)))
 
 
-def biquad_within_ref(got, x, coefs):
+def biquad_within_ref(got, x, coefs, truth=None, ref64=None):
     """Per channel: err_gpu <= max(4 err_ref64, 64 u rms(truth)), both errors against biquad_truth, err_ref64 that of
-    the reference's own FP64 recurrence (restate.biquad_cascade).  Returns per channel (err_gpu, err_ref64, ratio to
+    the reference's own FP64 recurrence (restate.biquad_cascade, or `ref64`: the reference library's output of the
+    same stream).  `truth` may be given when it is already known.  Returns per channel (err_gpu, err_ref64, ratio to
     the bound), errors relative to rms(truth); asserts the bound."""
     from oracle import restate
-    truth = biquad_truth(x, coefs)
-    ref64 = restate.biquad_cascade(x, coefs)
+    if truth is None:
+        truth = biquad_truth(x, coefs)
+    if ref64 is None:
+        ref64 = restate.biquad_cascade(x, coefs)
     out = []
     for c in range(x.shape[1]):
         t = truth[:, c]

@@ -103,3 +103,20 @@ def test_frontend_library_and_ladspa_plugin_load():
         env.setdefault("LADSPA_DSP_CONFIG_PATH", "/nonexistent")
         code = "import ctypes, sys; sys.exit(0 if hasattr(ctypes.CDLL(sys.argv[1]), 'ladspa_descriptor') else 1)"
         assert subprocess.run([sys.executable, "-c", code, plugin], env=env).returncode == 0
+
+
+def test_mirror_reads_numbers_as_strtod():
+    """dsp_b200.effects reads numeric words as the reference's strtod() + CHECK_ENDPTR do: decimal and hexadecimal
+    forms, inf and nan, and nothing after the number (Python's float() also takes digit separators, strtod() does not)."""
+    from dsp_b200.effects import ChainSyntaxError, parse_freq, parse_num, parse_width
+    for word, want in (("3", 3.0), ("-3.5", -3.5), ("+.5", 0.5), ("1.", 1.0), ("1e3", 1000.0), ("2.5E-1", 0.25),
+                       ("0x1.8p-1", 0.75), ("-0X10", -16.0), ("0x.8", 0.5), ("inf", float("inf")), ("-Infinity", float("-inf"))):
+        assert parse_num(word) == want, word
+    assert np.isnan(parse_num("nan")) and np.isnan(parse_num("NaN(1)"))
+    for word in ("1_000", "", "x", "1e", "0x", "1 ", "3dB", "0x1p", "infin", "1.2.3"):
+        with pytest.raises(ChainSyntaxError):
+            parse_num(word)
+    assert parse_freq("0x1p10k") == 1024000.0 and parse_width("0x1p1q") == (2.0, 1)
+    for word in ("1_0k", "1kk"):
+        with pytest.raises(ChainSyntaxError):
+            parse_freq(word)
