@@ -51,6 +51,7 @@
 #include "fft.cuh"
 #include "fir_pipe.cuh"
 #include "fir_plan.h"
+#include "fir_tile.cuh"
 #include "ops.h"
 #include <cooperative_groups.h>
 
@@ -220,22 +221,7 @@ __global__ void __launch_bounds__(FftCfg<N>::THREADS) k_fir_inv(InvArgs a)
 			w[i] = __ldg(&a.tw[k]);
 		}
 #pragma unroll
-		for (int i = 0; i < 8; ++i) {
-			const int k = t + i * T;
-			if (k == 0) {
-				// Z[0] = E0 + i O0 from the packed (DC, Nyquist) pair; Z[N/2] = conj(Y[N/2]); both stored conjugated
-				buf[0] = make_double2(0.5 * (yk[i].x + yk[i].y), -0.5 * (yk[i].x - yk[i].y));
-				buf[spad(N / 2)] = yn[i];
-			}
-			else {
-				const double2 e = make_double2(0.5 * (yk[i].x + yn[i].x), 0.5 * (yk[i].y - yn[i].y));
-				const double2 d = make_double2(0.5 * (yk[i].x - yn[i].x), 0.5 * (yk[i].y + yn[i].y));
-				const double2 o = cmul(cconj(w[i]), d);
-				// Z[k] = E + iO, Z[N-k] = conj(E) + i conj(O); store conj(Z)
-				buf[spad(k)] = make_double2(e.x - o.y, -(e.y + o.x));
-				buf[spad(N - k)] = make_double2(e.x + o.y, -(o.x - e.y));
-			}
-		}
+		for (int i = 0; i < 8; ++i) irfft_merge<N>(buf, t + i * T, N - (t + i * T), yk[i], yn[i], w[i]);
 	}
 	__syncthreads();
 	fft_forward_smem<N>(buf, a.ptw, t);
@@ -249,8 +235,8 @@ __global__ void __launch_bounds__(FftCfg<N>::THREADS) k_fir_inv(InvArgs a)
 			for (int i = 0; i < 8; ++i) {
 				const int n = t + i * T;
 				const double2 lo = buf[spad(n)], hi = buf[spad(n + N / 2)];
-				out[n] = make_double2(lo.x * scale, -lo.y * scale);
-				carry[n] = make_double2(hi.x * scale, -hi.y * scale);
+				out[n] = ola_scaled(lo, scale);
+				carry[n] = ola_scaled(hi, scale);
 			}
 			return;
 		}
@@ -262,8 +248,8 @@ __global__ void __launch_bounds__(FftCfg<N>::THREADS) k_fir_inv(InvArgs a)
 		for (int i = 0; i < 8; ++i) {
 			const int n = t + i * T;
 			const double2 lo = buf[spad(n)], hi = buf[spad(n + N / 2)];
-			if (a.flags & INV_OUT) out[n] = make_double2(fma(lo.x, scale, c[i].x), fma(-lo.y, scale, c[i].y));
-			if (a.flags & INV_UPDATE_CARRY) carry[n] = make_double2(hi.x * scale, -hi.y * scale);
+			if (a.flags & INV_OUT) out[n] = ola_out(lo, scale, c[i]);
+			if (a.flags & INV_UPDATE_CARRY) carry[n] = ola_scaled(hi, scale);
 		}
 	}
 }
@@ -302,18 +288,6 @@ struct L0Args {
 	int cluster_io;          // host: launch the CL variant (4 adjacent channels per cluster; needs xin and yout)
 };
 
-__device__ __forceinline__ void prefetch_l2(const void *p)
-{
-	asm volatile("prefetch.global.L2 [%0];" ::"l"(p));
-}
-
-// pull `bytes` starting at p towards L2, one request per 128-byte line, spread over the FFT's T threads
-__device__ __forceinline__ void prefetch_rows(const void *p, long bytes, int t, int T)
-{
-	const char *c = static_cast<const char *>(p);
-	for (long off = (long) t * 128; off < bytes; off += (long) T * 128) prefetch_l2(c + off);
-}
-
 // FIR_L0_ASYNC: the cluster form of the fused kernel exchanges its samples between the CTAs of a cluster with bulk
 // copies shared memory -> a neighbour's shared memory that complete bytes on the RECEIVER's mbarrier
 // (cp.async.bulk.shared::cluster.shared::cta), instead of plain distributed-shared-memory stores fenced by
@@ -341,56 +315,6 @@ struct L0ClCfg {
 	// the L1 (padding its shared memory alone slows it down).  After the buffers: two mbarriers.
 	static constexpr size_t SMEM = FIR_L0_ASYNC ? FftCfg<N>::SMEM + 16 : FftCfg<N>::SMEM;
 };
-
-__device__ __forceinline__ uint32_t mapa_u32(uint32_t cta_addr, uint32_t rank)
-{
-	uint32_t r;
-	asm volatile("mapa.shared::cluster.u32 %0, %1, %2;" : "=r"(r) : "r"(cta_addr), "r"(rank));
-	return r;
-}
-
-// `bytes` (a multiple of 16) from this CTA's shared memory into the shared memory of a CTA of the cluster; they count on
-// that CTA's mbarrier when they have landed.  Issued by one thread.
-__device__ __forceinline__ void bulk_s2c(uint32_t dst_cluster, uint32_t src_cta, unsigned bytes, uint32_t mbar_cluster)
-{
-	asm volatile("cp.async.bulk.shared::cluster.shared::cta.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];" ::"r"(dst_cluster), "r"(src_cta),
-	             "r"(bytes), "r"(mbar_cluster)
-	             : "memory");
-}
-
-// generic-proxy writes to shared memory before, async-proxy (bulk copy) reads of them after
-__device__ __forceinline__ void fence_proxy_async_smem()
-{
-	asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
-}
-
-// wait for a phase completed by other CTAs' bulk copies (acquire at cluster scope); traps instead of hanging
-__device__ __forceinline__ void mbar_wait_cluster(uint64_t *bar, unsigned parity)
-{
-	unsigned spins = 0;
-	for (;;) {
-		uint32_t ok;
-		asm volatile("{\n\t.reg .pred p;\n\tmbarrier.try_wait.parity.acquire.cluster.shared::cta.b64 p, [%1], %2;\n\tselp.u32 %0, 1, 0, p;\n\t}"
-		             : "=r"(ok)
-		             : "r"(smem_u32(bar)), "r"(parity)
-		             : "memory");
-		if (ok) return;
-		if (++spins > (1u << 20)) __trap();
-	}
-}
-
-// Cluster-wide execution barrier WITHOUT the release fence of cluster.sync(): for points where nothing written before
-// has to become visible to the other CTAs (the fence of the releasing form waits for every global store and prefetch
-// the thread still has in flight -- a third of the fused kernel's stall samples were that wait).
-__device__ __forceinline__ void cluster_barrier_relaxed()
-{
-	asm volatile("barrier.cluster.arrive.relaxed.aligned;\n\tbarrier.cluster.wait.aligned;" ::: "memory");
-}
-
-__device__ __forceinline__ double2 cmac(double2 acc, double2 x, double2 h)
-{
-	return make_double2(fma(x.x, h.x, fma(-x.y, h.y, acc.x)), fma(x.x, h.y, fma(x.y, h.x, acc.y)));
-}
 
 // CL: launched as clusters of 4 / CPB CTAs = 4 ADJACENT channels (four CTAs of one 4096- or 8192-point transform, two
 // CTAs of two 2048-point transforms) that do the direct-form I/O together: every CTA reads
@@ -475,25 +399,14 @@ __global__ void __launch_bounds__(FftCfg<N>::THREADS) __maxnreg__((N == 4096) ? 
 		else if (a.xin) {
 			// frames 2n, 2n+1 of this channel: 8-byte loads one row apart (the 3 neighbouring channels' CTAs use the
 			// rest of each sector at about the same time: L2 serves them)
-			const double *xc = a.xin + (a.xin_map ? a.xin_map[s] : s);
-#pragma unroll
-			for (int i = 0; i < 8; ++i) {
-				const long n2 = 2L * (t + i * T);
-				v[i] = make_double2(xc[n2 * a.xin_stride], xc[(n2 + 1) * a.xin_stride]);
-			}
+			read_frame_pairs<T>(v, a.xin + (a.xin_map ? a.xin_map[s] : s), a.xin_stride, t);
 		}
 		else {
 			const double2 *x = reinterpret_cast<const double2 *>(a.in + (long) s * a.in_ch_stride);
 #pragma unroll
 			for (int i = 0; i < 8; ++i) v[i] = x[t + i * T];
 		}
-		if constexpr (!(CL && FIR_L0_ASYNC)) {
-#pragma unroll
-			for (int i = 0; i < 8; ++i) {
-				if (!CL) buf[spad(t + i * T)] = v[i];
-				buf[spad(t + i * T + N / 2)] = make_double2(0.0, 0.0);
-			}
-		}
+		if constexpr (!(CL && FIR_L0_ASYNC)) fill_buf<N, T>(buf, CL ? nullptr : v, t);
 	}
 #if FIR_L0_ASYNC
 	if constexpr (CL) {
@@ -511,8 +424,7 @@ __global__ void __launch_bounds__(FftCfg<N>::THREADS) __maxnreg__((N == 4096) ? 
 		mbar_wait_cluster(&mbar[0], 0);   // the samples of this CTA's channels, from every CTA of the cluster
 		// every CTA has everything <=> every copy out of a staging area is complete: the second halves become zeros
 		cluster_barrier_relaxed();
-#pragma unroll
-		for (int i = 0; i < 8; ++i) buf[spad(t + i * T + N / 2)] = make_double2(0.0, 0.0);
+		fill_buf<N, T>(buf, nullptr, t);
 		__syncthreads();
 	}
 	else __syncthreads();
@@ -529,10 +441,7 @@ __global__ void __launch_bounds__(FftCfg<N>::THREADS) __maxnreg__((N == 4096) ? 
 			const double2 *fc_ = a.fdl + (long) s * a.fdl_ch_stride;
 			prefetch_rows(Hc, (long) P * N * sizeof(double2), t, T);
 #pragma unroll
-			for (int p = 1; p < P; ++p) {
-				const int sl = (a.slot - p < 0) ? a.slot - p + a.fdl_rows : a.slot - p;
-				prefetch_rows(fc_ + (long) sl * N, (long) N * sizeof(double2), t, T);
-			}
+			for (int p = 1; p < P; ++p) prefetch_rows(fc_ + (long) ring_back(a.slot, p, a.fdl_rows) * N, (long) N * sizeof(double2), t, T);
 			prefetch_rows(a.carry + (long) s * N, (long) N * sizeof(double), t, T);
 			if (a.init) prefetch_rows(a.init + (long) s * N, (long) N * sizeof(double2), t, T);
 		}
@@ -557,24 +466,11 @@ __global__ void __launch_bounds__(FftCfg<N>::THREADS) __maxnreg__((N == 4096) ? 
 #pragma unroll
 		for (int i = 0; i < 8; ++i) w[i] = __ldg(&a.tw[t + i * T]);
 #pragma unroll
-		for (int i = 0; i < 8; ++i) {
-			const int k = t + i * T;
-			if (k == 0) {
-				const double2 z0 = buf[0], zh = buf[spad(N / 2)];
-				const double2 x0 = make_double2(z0.x + z0.y, z0.x - z0.y), xh = cconj(zh);
-				X[0] = x0; X[N / 2] = xh;
-				buf[0] = x0; buf[spad(N / 2)] = xh;
-			}
-			else {
-				const double2 zk = buf[spad(k)], zn = buf[spad(N - k)];
-				const double2 e0 = make_double2(0.5 * (zk.x + zn.x), 0.5 * (zk.y - zn.y));
-				const double2 o0 = make_double2(0.5 * (zk.y + zn.y), -0.5 * (zk.x - zn.x));
-				const double2 wo = cmul(w[i], o0);
-				const double2 xk = cadd(e0, wo), xn = cconj(csub(e0, wo));
-				X[k] = xk; X[N - k] = xn;
-				buf[spad(k)] = xk; buf[spad(N - k)] = xn;
-			}
-		}
+		for (int i = 0; i < 8; ++i)
+			rfft_split<N>(buf, t + i * T, w[i], [&](int k, int n, double2 xk, double2 xn) {
+				X[k] = xk; X[n] = xn;
+				buf[spad(k)] = xk; buf[spad(n)] = xn;
+			});
 		// (2) S = X_j H_0 + sum_{p>=1} X_{j-p} H_p (+ Y_j) for the owned bins, one row (pair) at a time for all eight
 		//     bin pairs: 16 independent 16-byte loads in flight per pass instead of whatever fits next to the sums of
 		//     one bin pair -- the phase is a chain of memory round trips, nothing else.  The running sum is parked in
@@ -599,8 +495,7 @@ __global__ void __launch_bounds__(FftCfg<N>::THREADS) __maxnreg__((N == 4096) ? 
 			}
 		}
 		auto mac_partition = [&](int p) {
-			const int sl = (a.slot - p < 0) ? a.slot - p + a.fdl_rows : a.slot - p;
-			const double2 *Xp = fdl + (long) sl * N, *Hp = H + (long) p * N;
+			const double2 *Xp = fdl + (long) ring_back(a.slot, p, a.fdl_rows) * N, *Hp = H + (long) p * N;
 #pragma unroll
 			for (int half = 0; half < 8; half += 4) {
 				double2 xk[4], xn[4], hk[4], hn[4];
@@ -616,8 +511,7 @@ __global__ void __launch_bounds__(FftCfg<N>::THREADS) __maxnreg__((N == 4096) ? 
 				for (int i = 0; i < 4; ++i) {
 					const int k = L0_K(half + i), n = L0_N(half + i);
 					double2 Sk = buf[spad(k)];
-					if (k == 0) { Sk.x = fma(xk[i].x, hk[i].x, Sk.x); Sk.y = fma(xk[i].y, hk[i].y, Sk.y); }
-					else Sk = cmac(Sk, xk[i], hk[i]);
+					cmac_packed(Sk, xk[i], hk[i], k == 0);
 					buf[spad(k)] = Sk;
 					buf[spad(n)] = cmac(buf[spad(n)], xn[i], hn[i]);
 				}
@@ -655,17 +549,7 @@ __global__ void __launch_bounds__(FftCfg<N>::THREADS) __maxnreg__((N == 4096) ? 
 					Sk = cadd(Sk, yk[i]);
 					Sn = cadd(Sn, yn[i]);
 				}
-				if (k == 0) {
-					buf[0] = make_double2(0.5 * (Sk.x + Sk.y), -0.5 * (Sk.x - Sk.y));
-					buf[spad(N / 2)] = Sn;   // conj(Z[N/2]) = S[N/2]
-				}
-				else {
-					const double2 e = make_double2(0.5 * (Sk.x + Sn.x), 0.5 * (Sk.y - Sn.y));
-					const double2 d = make_double2(0.5 * (Sk.x - Sn.x), 0.5 * (Sk.y + Sn.y));
-					const double2 o = cmul(cconj(w2[i]), d);
-					buf[spad(k)] = make_double2(e.x - o.y, -(e.y + o.x));
-					buf[spad(n)] = make_double2(e.x + o.y, -(o.x - e.y));
-				}
+				irfft_merge<N>(buf, k, n, Sk, Sn, w2[i]);
 			}
 		}
 #undef L0_K
@@ -685,14 +569,10 @@ __global__ void __launch_bounds__(FftCfg<N>::THREADS) __maxnreg__((N == 4096) ? 
 		for (int i = 0; i < 8; ++i) {
 			const int n = t + i * T;
 			const double2 lo = buf[spad(n)], hi = buf[spad(n + N / 2)];
-			const double2 y = make_double2(fma(lo.x, scale, c[i].x), fma(-lo.y, scale, c[i].y));
+			const double2 y = ola_out(lo, scale, c[i]);
 			if (CL) {
-#if FIR_L0_ASYNC
 				buf[spad(n)] = y;   // this thread is the only one that touches entry n after the last pass
-				carry[n] = make_double2(hi.x * scale, -hi.y * scale);
-#else
-				buf[spad(n)] = y;   // this thread is the only one that touches entry n after the last pass
-#endif
+				if (FIR_L0_ASYNC) carry[n] = ola_scaled(hi, scale);
 			}
 			else if (yc) {
 				yc[2L * n * a.yout_stride] = y.x;
@@ -701,7 +581,7 @@ __global__ void __launch_bounds__(FftCfg<N>::THREADS) __maxnreg__((N == 4096) ? 
 			else out[n] = y;
 			// (cluster form with fenced barriers: the new carry is stored after the barrier below -- its release fence
 			// would wait for these stores; the second half of the buffer, where it comes from, is nobody else's)
-			if (!CL) carry[n] = make_double2(hi.x * scale, -hi.y * scale);
+			if (!CL) carry[n] = ola_scaled(hi, scale);
 		}
 	}
 	if constexpr (CL) {
@@ -754,11 +634,7 @@ __global__ void __launch_bounds__(FftCfg<N>::THREADS) __maxnreg__((N == 4096) ? 
 			const double scale = 1.0 / N;
 			double2 *carry = reinterpret_cast<double2 *>(a.carry + (long) s * N);
 #pragma unroll
-			for (int i = 0; i < 8; ++i) {
-				const int n = t + i * T;
-				const double2 hi = buf[spad(n + N / 2)];
-				carry[n] = make_double2(hi.x * scale, -hi.y * scale);
-			}
+			for (int i = 0; i < 8; ++i) carry[t + i * T] = ola_scaled(buf[spad(t + i * T + N / 2)], scale);
 		}
 		cluster_barrier_relaxed();   // nobody leaves while its buffer may still be read (execution only: nothing to publish)
 #endif
@@ -895,9 +771,7 @@ __device__ __forceinline__ void fir_mac_batch_body(const MacBatchArgs &a, int y)
 	const bool dc = DCW && (k == 0);
 	const double2 zero = make_double2(0.0, 0.0);
 	double2 acc[T], hw[T];
-	// A row meets only the filter rows of its window: bit t of `live` says whether hw[t] is one.  The products with the
-	// others are skipped, not multiplied by zero -- an FDL row outside period t's window may hold a NaN or Inf (of a
-	// block this period does not depend on), and 0 x NaN would carry it into V_j.
+	// bit t of `live`: hw[t] is a filter row of period t's window (the NaN rule: window_mac())
 #define HLIVE(p) ((p) >= a.p_lo && (p) < h_hi)
 #define HROW(p) (HLIVE(p) ? (SHARED_H ? __ldg(&H[(long) (p) * a.N]) : __ldcs(&H[(long) (p) * a.N])) : zero)
 	int m = a.pf + 1;   // first row: the newest complete block, X_q
@@ -913,17 +787,7 @@ __device__ __forceinline__ void fir_mac_batch_body(const MacBatchArgs &a, int y)
 #define XROW(d) __ldcs(&fdl[(long) ((slot - (d) < 0) ? slot - (d) + a.P : slot - (d)) * a.N])
 #define STEP(XV, HN, PN)                                                      \
 	do {                                                                      \
-		_Pragma("unroll") for (int t = 0; t < T; ++t) {                       \
-			if (!((live >> t) & 1u)) continue;                                \
-			if (dc) {                                                         \
-				acc[t].x = fma(XV.x, hw[t].x, acc[t].x);                      \
-				acc[t].y = fma(XV.y, hw[t].y, acc[t].y);                      \
-			}                                                                 \
-			else {                                                            \
-				acc[t].x = fma(XV.x, hw[t].x, fma(-XV.y, hw[t].y, acc[t].x)); \
-				acc[t].y = fma(XV.x, hw[t].y, fma(XV.y, hw[t].x, acc[t].y));  \
-			}                                                                 \
-		}                                                                     \
+		window_mac<T>(acc, hw, live, XV, dc);                                 \
 		_Pragma("unroll") for (int t = 0; t + 1 < T; ++t) hw[t] = hw[t + 1];  \
 		hw[T - 1] = HN;                                                       \
 		live = (live >> 1) | ((unsigned) HLIVE(PN) << (T - 1));               \
@@ -1077,9 +941,8 @@ __global__ void __launch_bounds__(256) k_fir_mac_bulk(MacBulkArgs a)
 	const bool dc = (k == 0);
 	const double2 zero = make_double2(0.0, 0.0);
 	double2 acc[T], hw[T];
-	// bit i of `live`: hw[i] is a filter row (0 <= d + i < P).  Products with the others are skipped, not multiplied by
-	// zero: the row of a later block of this call (or a stale row past the new ones) may hold a NaN or Inf, and 0 x NaN
-	// would carry it into the outputs of earlier blocks.
+	// bit i of `live`: hw[i] is a filter row (0 <= d + i < P); the NaN rule (window_mac()) keeps a NaN or Inf in the row
+	// of a later block of this call (or a stale row past the new ones) out of the outputs of earlier blocks
 #define HLIVE(p) ((p) >= 0 && (p) < a.P)
 #define HROW(p) (HLIVE(p) ? (SHARED_H ? __ldg(&H[(long) (p) * a.N]) : __ldcs(&H[(long) (p) * a.N])) : zero)
 	// step d = P-1 .. -(T-1): block m = j - d meets H_{d+i} for output i; window hw[i] = H_{d+i}
@@ -1095,17 +958,7 @@ __global__ void __launch_bounds__(256) k_fir_mac_bulk(MacBulkArgs a)
 #define XROW(e) __ldcs(&fdl[(long) ((slot + (e) >= a.rows) ? slot + (e) - a.rows : slot + (e)) * a.N])
 #define STEP(XV, HN, PN)                                                      \
 	do {                                                                      \
-		_Pragma("unroll") for (int i = 0; i < T; ++i) {                       \
-			if (!((live >> i) & 1u)) continue;                                \
-			if (dc) {                                                         \
-				acc[i].x = fma(XV.x, hw[i].x, acc[i].x);                      \
-				acc[i].y = fma(XV.y, hw[i].y, acc[i].y);                      \
-			}                                                                 \
-			else {                                                            \
-				acc[i].x = fma(XV.x, hw[i].x, fma(-XV.y, hw[i].y, acc[i].x)); \
-				acc[i].y = fma(XV.x, hw[i].y, fma(XV.y, hw[i].x, acc[i].y));  \
-			}                                                                 \
-		}                                                                     \
+		window_mac<T>(acc, hw, live, XV, dc);                                 \
 		_Pragma("unroll") for (int i = T - 1; i > 0; --i) hw[i] = hw[i - 1];  \
 		hw[0] = HN;                                                           \
 		live = ((live << 1) | (unsigned) HLIVE(PN)) & ((1u << T) - 1);        \

@@ -28,6 +28,7 @@
 #include "common.cuh"
 #include "fft.cuh"
 #include "fir_plan.h"
+#include "fir_tile.cuh"
 #include <cstdint>
 
 namespace dspb200 {
@@ -91,95 +92,6 @@ enum {
 	PC_EXIT = 512
 };
 
-// ---- mbarrier / bulk-copy primitives (PTX; SASS: SYNCS.*, UBLKCP) -------------------------------------------
-__device__ __forceinline__ uint32_t smem_u32(const void *p) { return (uint32_t) __cvta_generic_to_shared(p); }
-
-__device__ __forceinline__ void mbar_init(uint64_t *bar, unsigned count)
-{
-	asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(smem_u32(bar)), "r"(count) : "memory");
-}
-
-__device__ __forceinline__ void mbar_arrive(uint64_t *bar)
-{
-	asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(smem_u32(bar)) : "memory");
-}
-
-__device__ __forceinline__ void mbar_arrive_expect_tx(uint64_t *bar, unsigned bytes)
-{
-	asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(smem_u32(bar)), "r"(bytes) : "memory");
-}
-
-__device__ __forceinline__ bool mbar_try_wait(uint64_t *bar, unsigned parity)
-{
-	uint32_t ok;
-	asm volatile("{\n\t.reg .pred p;\n\tmbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2;\n\tselp.u32 %0, 1, 0, p;\n\t}"
-	             : "=r"(ok)
-	             : "r"(smem_u32(bar)), "r"(parity)
-	             : "memory");
-	return ok != 0;
-}
-
-// non-blocking probe (the MAC warps look at the NEXT stage before they work on the current one: its latency hides
-// behind the arithmetic)
-__device__ __forceinline__ bool mbar_test_wait(uint64_t *bar, unsigned parity)
-{
-	uint32_t ok;
-	asm volatile("{\n\t.reg .pred p;\n\tmbarrier.test_wait.parity.shared::cta.b64 p, [%1], %2;\n\tselp.u32 %0, 1, 0, p;\n\t}"
-	             : "=r"(ok)
-	             : "r"(smem_u32(bar)), "r"(parity)
-	             : "memory");
-	return ok != 0;
-}
-
-// one lane of a converged warp (ptxas then knows the code under it is executed by a single thread: the bulk copies
-// are issued straight from uniform registers instead of a per-lane loop)
-__device__ __forceinline__ bool elect_one()
-{
-	uint32_t pred;
-	asm volatile("{\n\t.reg .pred p;\n\telect.sync _|p, 0xffffffff;\n\tselp.u32 %0, 1, 0, p;\n\t}" : "=r"(pred));
-	return pred != 0;
-}
-
-// try_wait suspends the warp in hardware for a bounded time; a wait that has not come true after 2^20 of them (>= 50 ms) is a
-// protocol bug: trap (the launch fails with an error) rather than hang the device
-__device__ __forceinline__ void mbar_wait(uint64_t *bar, unsigned parity)
-{
-	unsigned spins = 0;
-	while (!mbar_try_wait(bar, parity))
-		if (++spins > (1u << 20)) __trap();
-}
-
-__device__ __forceinline__ uint64_t l2_policy_evict_first()
-{
-	uint64_t pol;
-	asm volatile("createpolicy.fractional.L2::evict_first.b64 %0, 1.0;" : "=l"(pol));
-	return pol;
-}
-
-// global -> shared bulk copy, completion signalled on `bar` in bytes
-__device__ __forceinline__ void bulk_g2s(void *dst, const void *src, unsigned bytes, uint64_t *bar, bool hint, uint64_t pol)
-{
-	if (hint)
-		asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes.L2::cache_hint [%0], [%1], %2, [%3], %4;" ::"r"(smem_u32(dst)),
-		             "l"(src), "r"(bytes), "r"(smem_u32(bar)), "l"(pol)
-		             : "memory");
-	else
-		asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];" ::"r"(smem_u32(dst)), "l"(src),
-		             "r"(bytes), "r"(smem_u32(bar))
-		             : "memory");
-}
-
-__device__ __forceinline__ double2 pipe_cmac(double2 acc, double2 x, double2 h)
-{
-	return make_double2(fma(x.x, h.x, fma(-x.y, h.y, acc.x)), fma(x.x, h.y, fma(x.y, h.x, acc.y)));
-}
-
-__device__ __forceinline__ void pipe_prefetch_rows(const void *p, long bytes, int t, int T)
-{
-	const char *c = static_cast<const char *>(p);
-	for (long off = (long) t * 128; off < bytes; off += (long) T * 128) asm volatile("prefetch.global.L2 [%0];" ::"l"(c + off));
-}
-
 // Register cap: the register file is split over the SM's four sub-partitions (16384 each) and a CTA's warps are dealt
 // round-robin: 13 warps = at most 4 per sub-partition = 128 registers per thread (a 17-warp layout with 8 MAC warps
 // would have to fit 5 x 32 x R <= 16384, i.e. 96 registers, which the transform team cannot live with).
@@ -233,19 +145,11 @@ __global__ void __maxnreg__(FIR_PIPE_MAXNREG) k_fir_pipe(PipeArgs a)
 				const double *xc = a.fake_io ? a.xin + (long) s * N : a.xin + (a.xin_map ? a.xin_map[s] : s);
 				const long xs = a.fake_io ? 1 : a.xin_stride;
 				double2 v[8];
-#pragma unroll
-				for (int i = 0; i < 8; ++i) {
-					const long n2 = 2L * (t + i * T);
-					v[i] = make_double2(xc[n2 * xs], xc[(n2 + 1) * xs]);   // plain loads: the call may be in place
-				}
+				read_frame_pairs<T>(v, xc, xs, t);   // plain loads: the call may be in place
 				// what the later phases read with plain loads: on its way to L2 while the first transform runs
-				pipe_prefetch_rows(H0, (long) N * sizeof(double2), t, T);
-				pipe_prefetch_rows(carry, (long) N * sizeof(double), t, T);
-#pragma unroll
-				for (int i = 0; i < 8; ++i) {
-					buf[spad(t + i * T)] = v[i];
-					buf[spad(t + i * T + N / 2)] = make_double2(0.0, 0.0);
-				}
+				prefetch_rows(H0, (long) N * sizeof(double2), t, T);
+				prefetch_rows(carry, (long) N * sizeof(double), t, T);
+				fill_buf<N, T>(buf, v, t);
 			}
 			TeamSync::sync();
 			fft_forward_smem<N, TeamSync>(buf, a.ptw, t);
@@ -255,24 +159,11 @@ __global__ void __maxnreg__(FIR_PIPE_MAXNREG) k_fir_pipe(PipeArgs a)
 			// (1) real split: X[k], X[N-k] to the FDL and, in place of Z, to shared memory.
 			//     Thread t owns the pairs k = t + i T; thread 0 also owns k = 0 (packed DC/Nyquist) and k = N/2.
 #pragma unroll
-			for (int i = 0; i < 8; ++i) {
-				const int k = t + i * T;
-				if (k == 0) {
-					const double2 z0 = buf[0], zh = buf[spad(N / 2)];
-					const double2 x0 = make_double2(z0.x + z0.y, z0.x - z0.y), xh = cconj(zh);
-					X[0] = x0; X[N / 2] = xh;
-					buf[0] = x0; buf[spad(N / 2)] = xh;
-				}
-				else {
-					const double2 zk = buf[spad(k)], zn = buf[spad(N - k)];
-					const double2 e0 = make_double2(0.5 * (zk.x + zn.x), 0.5 * (zk.y - zn.y));
-					const double2 o0 = make_double2(0.5 * (zk.y + zn.y), -0.5 * (zk.x - zn.x));
-					const double2 wo = cmul(w[i], o0);
-					const double2 xk = cadd(e0, wo), xn = cconj(csub(e0, wo));
-					X[k] = xk; X[N - k] = xn;
-					buf[spad(k)] = xk; buf[spad(N - k)] = xn;
-				}
-			}
+			for (int i = 0; i < 8; ++i)
+				rfft_split<N>(buf, t + i * T, w[i], [&](int k, int n, double2 xk, double2 xn) {
+					X[k] = xk; X[n] = xn;
+					buf[spad(k)] = xk; buf[spad(n)] = xn;
+				});
 			// (2) S = X_j H_0 + (what the MAC warps summed for this channel), inverse merge into shared memory
 			{
 				const long long t0 = stats_on ? clock64() : 0;
@@ -286,20 +177,9 @@ __global__ void __maxnreg__(FIR_PIPE_MAXNREG) k_fir_pipe(PipeArgs a)
 				const double2 xk = buf[spad(k)], xn = buf[spad(n)];
 				const double2 hk = __ldg(&H0[k]), hn = __ldg(&H0[n]);
 				double2 Sk = sbuf[k], Sn = sbuf[n];
-				if (k == 0) { Sk.x = fma(xk.x, hk.x, Sk.x); Sk.y = fma(xk.y, hk.y, Sk.y); }   // packed bin: two real products
-				else Sk = pipe_cmac(Sk, xk, hk);
-				Sn = pipe_cmac(Sn, xn, hn);
-				if (k == 0) {
-					buf[0] = make_double2(0.5 * (Sk.x + Sk.y), -0.5 * (Sk.x - Sk.y));
-					buf[spad(N / 2)] = Sn;   // conj(Z[N/2]) = S[N/2]
-				}
-				else {
-					const double2 e = make_double2(0.5 * (Sk.x + Sn.x), 0.5 * (Sk.y - Sn.y));
-					const double2 d = make_double2(0.5 * (Sk.x - Sn.x), 0.5 * (Sk.y + Sn.y));
-					const double2 o = cmul(cconj(w[i]), d);
-					buf[spad(k)] = make_double2(e.x - o.y, -(e.y + o.x));
-					buf[spad(n)] = make_double2(e.x + o.y, -(o.x - e.y));
-				}
+				cmac_packed(Sk, xk, hk, k == 0);
+				Sn = cmac(Sn, xn, hn);
+				irfft_merge<N>(buf, k, n, Sk, Sn, w[i]);
 			}
 			__syncwarp();
 			if (lane == 0) mbar_arrive(s_empty);   // sbuf may be refilled for the next channel
@@ -317,9 +197,10 @@ __global__ void __maxnreg__(FIR_PIPE_MAXNREG) k_fir_pipe(PipeArgs a)
 				for (int i = 0; i < 8; ++i) {
 					const int n = t + i * T;
 					const double2 lo = buf[spad(n)], hi = buf[spad(n + N / 2)];
-					yc[2L * n * ys] = fma(lo.x, scale, c[i].x);
-					yc[(2L * n + 1) * ys] = fma(-lo.y, scale, c[i].y);
-					carry[n] = make_double2(hi.x * scale, -hi.y * scale);
+					const double2 y = ola_out(lo, scale, c[i]);
+					yc[2L * n * ys] = y.x;
+					yc[(2L * n + 1) * ys] = y.y;
+					carry[n] = ola_scaled(hi, scale);
 				}
 			}
 			// entry n and n + N/2 of buf are only touched by this thread between the last pass and the next
@@ -339,9 +220,7 @@ __global__ void __maxnreg__(FIR_PIPE_MAXNREG) k_fir_pipe(PipeArgs a)
 		unsigned phase = 0;
 		const double2 zero = make_double2(0.0, 0.0);
 		double2 accS[PER], accB[TB][PER], hw[TB][PER];
-		// bit u: hw[u] is a filter row of the batch window; products with the zero rows around it are skipped, so that a
-		// NaN or Inf in an FDL row outside a period's window stays out of that period's V (0 x NaN = NaN)
-		unsigned liveB = 0;
+		unsigned liveB = 0;   // bit u: hw[u] is a filter row of the batch window (window_mac())
 #pragma unroll
 		for (int i = 0; i < PER; ++i) {
 			accS[i] = zero;
@@ -368,19 +247,9 @@ __global__ void __maxnreg__(FIR_PIPE_MAXNREG) k_fir_pipe(PipeArgs a)
 				for (int i = 0; i < PER; ++i) {
 					const double2 x = Xs[tm + i * TM];
 					const double2 hn = (fl & PC_BHASH) ? Hs[tm + i * TM] : zero;
-					if (dc && i == 0) {
-#pragma unroll
-						for (int u = 0; u < TB; ++u) {
-							if (!((liveB >> u) & 1u)) continue;
-							accB[u][i].x = fma(x.x, hw[u][i].x, accB[u][i].x);
-							accB[u][i].y = fma(x.y, hw[u][i].y, accB[u][i].y);
-						}
-					}
-					else {
-#pragma unroll
-						for (int u = 0; u < TB; ++u)
-							if ((liveB >> u) & 1u) accB[u][i] = pipe_cmac(accB[u][i], x, hw[u][i]);
-					}
+					// two calls with a constant dc, as the kernel had them (one call with dc && i == 0 compiles to other code)
+					if (dc && i == 0) window_mac<TB, PER>(&accB[0][i], &hw[0][i], liveB, x, true);
+					else window_mac<TB, PER>(&accB[0][i], &hw[0][i], liveB, x, false);
 #pragma unroll
 					for (int u = 0; u + 1 < TB; ++u) hw[u][i] = hw[u + 1][i];
 					hw[TB - 1][i] = hn;
@@ -404,13 +273,9 @@ __global__ void __maxnreg__(FIR_PIPE_MAXNREG) k_fir_pipe(PipeArgs a)
 #pragma unroll
 					for (int i = 0; i < PER; ++i) accS[i] = zero;
 				}
-				if (dc) {
-					accS[0].x = fma(x[0].x, h[0].x, accS[0].x);
-					accS[0].y = fma(x[0].y, h[0].y, accS[0].y);
-				}
-				else accS[0] = pipe_cmac(accS[0], x[0], h[0]);
+				cmac_packed(accS[0], x[0], h[0], dc);
 #pragma unroll
-				for (int i = 1; i < PER; ++i) accS[i] = pipe_cmac(accS[i], x[i], h[i]);
+				for (int i = 1; i < PER; ++i) accS[i] = cmac(accS[i], x[i], h[i]);
 				if (fl & PC_SSTORE) {
 #pragma unroll
 					for (int i = 0; i < PER; ++i) sbuf[chunk * CHUNK + tm + i * TM] = accS[i];
