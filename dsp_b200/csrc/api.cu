@@ -454,6 +454,8 @@ void dspb200_profile_enable(int on) { g_profile_on.store(on ? 1 : 0); }
 
 void dspb200_debug_serialize(int on) { fir_debug_serialize(on); }
 
+int dspb200_debug_stall(int roles, int microseconds, int period, int phase) { return fir_debug_stall(roles, microseconds, period, phase); }
+
 int dspb200_profile_read(const char *name, double *total_ms, long *launches)
 {
 	std::lock_guard<std::mutex> lk(g_prof_lock);

@@ -53,11 +53,32 @@
 #include "fir_plan.h"
 #include "fir_tile.cuh"
 #include "ops.h"
+#include "../../include/dsp_b200.h"
 #include <cooperative_groups.h>
 
 namespace dspb200 {
 
 std::atomic<int> g_fir_serialize{0};   // dspb200_debug_serialize(): no side streams (isolated kernel timings)
+
+// dspb200_debug_stall(): a FirOp puts a delay kernel on each selected stream of its blocks blk % period == phase, right
+// before that stream's first FIR launch of the block, so that the stream falls behind the others.  Packed in one word
+// (roles | microseconds << 8 | period << 24 | phase << 44), read with one relaxed load per block; 0: off.
+std::atomic<unsigned long long> g_fir_stall{0};
+constexpr int FIR_STALL_MAX_US = 5000;
+
+struct FirStall {
+	int roles = 0, us = 0;
+	long period = 1, phase = 0;
+	static FirStall load()
+	{
+		const unsigned long long w = g_fir_stall.load(std::memory_order_relaxed);
+		FirStall s;
+		if (!w) return s;
+		s.roles = (int) (w & 0xff); s.us = (int) ((w >> 8) & 0xffff); s.period = (long) ((w >> 24) & 0xfffff); s.phase = (long) (w >> 44);
+		return s;
+	}
+	bool hits(int role, long blk) const { return (roles & role) && blk % period == phase; }
+};
 
 template <int... N> constexpr bool fft_cpb_matches() { return ((fir_fft_cpb(N) == FftCfg<N>::CPB) && ...); }
 static_assert(fft_cpb_matches<64, 128, 256, 512, 1024, 2048, 4096, 8192>(), "fir_plan.h's fir_fft_cpb() is FftCfg<N>::CPB");
@@ -641,6 +662,19 @@ __global__ void __launch_bounds__(FftCfg<N>::THREADS) __maxnreg__((N == 4096) ? 
 	}
 }
 
+// dspb200_debug_stall(): one thread waits `ns` nanoseconds of %globaltimer (at most FIR_STALL_MAX_US) and ends; the
+// iteration cap bounds the loop whatever the timer does
+__global__ void k_fir_stall(long long ns)
+{
+	unsigned long long t0, t;
+	asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t0));
+	for (int i = 0; i < (1 << 18); ++i) {
+		asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t));
+		if ((long long) (t - t0) >= ns) break;
+		__nanosleep(256);
+	}
+}
+
 // Y[s][k] = sum_{p in [p0,p1)} FDL[s][(slot0 - p) mod P][k] * H[s or 0][p][k]   (packed bin 0)
 // The HBM-streaming kernel of the engine: 32 bytes in per complex MAC (16 with a shared IR, whose
 // rows stay in L2), 4 DFMA.
@@ -1209,6 +1243,18 @@ static void launch_mac(const MacArgs &a, int n_sel, bool shared_h, const char *p
 // ------------------------------------------------------------------------------------------
 void fir_debug_serialize(int on) { g_fir_serialize.store(on ? 1 : 0); }
 
+int fir_debug_stall(int roles, int us, int period, int phase)
+{
+	const int all = DSPB200_STALL_MAIN | DSPB200_STALL_SIDE | DSPB200_STALL_SIDE2 | DSPB200_STALL_HOT;
+	if (roles & ~all || us < 0 || us > FIR_STALL_MAX_US || period < 1 || period > 0xfffff || phase < 0 || phase >= period) {
+		set_error("debug_stall: roles %d, %d us (at most %d), period %d, phase %d", roles, us, FIR_STALL_MAX_US, period, phase);
+		return -1;
+	}
+	g_fir_stall.store(roles ? (unsigned long long) roles | (unsigned long long) us << 8 | (unsigned long long) period << 24 |
+	                          (unsigned long long) phase << 44 : 0ULL);
+	return 0;
+}
+
 int test_rfft(int B, int n_ch, const double *d_in, double *d_spec, cudaStream_t st)
 {
 	FwdArgs a = {};
@@ -1307,6 +1353,15 @@ struct FirOp : Op {
 	// (per-channel form / cluster form), the pipeline kernel, the bulk form and the general path (forward, MAC, inverse),
 	// and launches of the head kernel (ragged calls)
 	long n_fused = 0, n_cluster = 0, n_pipe = 0, n_bulk = 0, n_general = 0, n_head = 0;
+	FirStall stall;   // dspb200_debug_stall() as it was at the start of the current level-0 block
+
+	// the test hook's delay on stream `st` (role DSPB200_STALL_*) before its first FIR launch of level-0 block `blk`
+	void stall_on(int role, long blk, cudaStream_t st)
+	{
+		if (!stall.hits(role, blk)) return;
+		ProfScope prof("fir_stall", st);
+		LAUNCH(k_fir_stall, 1, 1, 0, st, (long long) stall.us * 1000);
+	}
 
 	const char *name() const override { return "fir"; }
 
@@ -1529,6 +1584,7 @@ struct FirOp : Op {
 			if (!any && us != st) {
 				CUDA_TRY(cudaEventRecord(ev_main, st), return -1);
 				CUDA_TRY(cudaStreamWaitEvent(side, ev_main, 0), return -1);
+				stall_on(DSPB200_STALL_SIDE, lv[0].blk - 1, side);
 			}
 			any = true;
 			L0Args f = {};
@@ -1557,6 +1613,7 @@ struct FirOp : Op {
 			if (tl.n > 0) {
 				// X_q is in the FDL once the partition-0 kernel of this block has run (ev_urgent on the side stream)
 				CUDA_TRY(cudaStreamWaitEvent(bs, ev_urgent, 0), return -1);
+				if (bs != st) stall_on(DSPB200_STALL_SIDE2, lv[0].blk - 1, bs);
 				const int threads = (Lp.B < batch_threads_for(s.t_batch)) ? Lp.B : batch_threads_for(s.t_batch);
 				launch_mac_batch(s.t_batch, fc == 1, dim3(Lp.B / threads, n_sel), threads, bs, batch_args(tl.l[0], q));
 				CUDA_TRY(cudaEventRecord(ev_batch[(q / s.t_batch) & 1], bs), return -1);
@@ -1631,6 +1688,7 @@ struct FirOp : Op {
 			ta.b = batch_args(tl.l[0], q);
 			ta.n_batch_y = tl.l[0].rows;
 			const dim3 grid(Lp.B / 256, ta.n_batch_y + n_sel);
+			if (!on_main) stall_on(DSPB200_STALL_SIDE, q, ts);
 			{
 				ProfScope prof("fir_tail", ts);
 				if (fc == 1) LAUNCH((k_fir_tail<4, true>), grid, 256, 0, ts, ta);
@@ -1644,6 +1702,7 @@ struct FirOp : Op {
 		}
 		// the tier launches up to block q-1 = tier_wait(j): every one made so far
 		if (s.t_batch > 0 && ev_bs_last) CUDA_TRY(cudaStreamWaitEvent(ts, ev_bs_last, 0), return -1);
+		if (!on_main) stall_on(DSPB200_STALL_SIDE, q, ts);
 		mac(0, s.mac_parts().first, s.mac_parts().second, j, ts, Y, (s.t_batch > 0) ? d_V + (size_t) (j % (2 * s.t_batch)) * n_sel * Lp.B : nullptr);
 		CUDA_TRY(cudaEventRecord(ev_tail[j & 1], ts), return -1);
 		if (s.t_batch > 0 && launch_tiers0(q, bs, serial)) return -1;
@@ -1658,7 +1717,10 @@ struct FirOp : Op {
 		for (int i = 0; i < tl.n; ++i) {
 			const FirTierLaunch &d = tl.l[i];
 			if (d.rows + d.pass_rows == 0) continue;
-			if (!any && !serial) CUDA_TRY(cudaStreamWaitEvent(bs, ev_main, 0), return -1);
+			if (!any && !serial) {
+				CUDA_TRY(cudaStreamWaitEvent(bs, ev_main, 0), return -1);
+				stall_on(DSPB200_STALL_SIDE2, q, bs);
+			}
 			any = true;
 			int threads = batch_threads_for(d.T);
 			if ((batch_threads == 128 || batch_threads == 64) && batch_threads < threads) threads = batch_threads;
@@ -1859,6 +1921,10 @@ struct FirOp : Op {
 		while (done < frames) {
 			const double *src = in + done * C;
 			double *d = dst + done * dstride;
+			if (abs_pos % s.B0 == 0) {
+				stall = FirStall::load();
+				stall_on(DSPB200_STALL_MAIN, L0.blk, st);
+			}
 			if (s.nb_max > 1 && abs_pos % s.B0 == 0 && frames - done >= 2L * s.B0) {
 				long nb = (frames - done) / s.B0;
 				if (nb > s.nb_max) nb = s.nb_max;
@@ -1941,6 +2007,7 @@ struct FirOp : Op {
 						CUDA_TRY(cudaStreamWaitEvent(ls, ev_tail[L0.blk & 1], 0), return -1);
 						f.init = d_Y_side + (size_t) (L0.blk & 1) * n_sel * s.B0;
 					}
+					if (use_hot) stall_on(DSPB200_STALL_HOT, L0.blk, hot);
 					if (launch_level0(s.B0, f, ls)) return -1;
 					if (use_hot) {
 						CUDA_TRY(cudaEventRecord(ev_hot_out, hot), return -1);

@@ -25,6 +25,7 @@ struct ResampleParams;
 int resample_params_or_error(int fs_in, int fs_out, double bw, ResampleParams *p);
 
 void fir_debug_serialize(int on);
+int fir_debug_stall(int roles, int us, int period, int phase);
 int test_rfft(int B, int n_ch, const double *d_in, double *d_spec, cudaStream_t st);
 int test_irfft(int B, int n_ch, const double *d_spec, double *d_out2B, cudaStream_t st);
 

@@ -29,6 +29,7 @@ SIGNATURES = {
     "dspb200_kernel_launches": (C.c_longlong, []),
     "dspb200_profile_enable": (None, [C.c_int]),
     "dspb200_debug_serialize": (None, [C.c_int]),
+    "dspb200_debug_stall": (C.c_int, [C.c_int, C.c_int, C.c_int, C.c_int]),
     "dspb200_profile_read": (C.c_int, [C.c_char_p, C.POINTER(C.c_double), _lp]),
     "dspb200_chain_create": (C.c_void_p, [C.c_int, C.c_int, _ip, C.c_int, C.c_int]),
     "dspb200_chain_destroy": (None, [C.c_void_p]),
@@ -100,6 +101,16 @@ def profile_enable(on):
 
 def debug_serialize(on):
     lib().dspb200_debug_serialize(1 if on else 0)
+
+
+# roles of debug_stall (DSPB200_STALL_* in include/dsp_b200.h)
+STALL_MAIN, STALL_SIDE, STALL_SIDE2, STALL_HOT = 1, 2, 4, 8
+
+
+def debug_stall(roles, microseconds=0, period=1, phase=0):
+    """Test aid: FIR operators delay the streams in `roles` by `microseconds` before their first FIR launch of every
+    level-0 block blk % period == phase (roles = 0: off).  Results must not change."""
+    _check(lib().dspb200_debug_stall(int(roles), int(microseconds), int(period), int(phase)), "debug_stall")
 
 
 def profile_read(name):

@@ -58,6 +58,14 @@ int  dspb200_profile_read(const char *name, double *total_ms, long *launches);
 /* Measurement aid: while on, operators that normally overlap work on side streams enqueue everything on the
  * caller's stream, so per-kernel durations are free of contention (results are identical either way). */
 void dspb200_debug_serialize(int on);
+/* Test aid for the FIR's cross-stream ordering: while `roles` is non-zero, an FIR operator enqueues a delay of
+ * `microseconds` (at most 5000) on each selected stream of its level-0 blocks blk % period == phase, right before that
+ * stream's first FIR launch of the block, so that the stream falls behind the others.  Roles: the caller's stream (or
+ * the shard's), the side stream (upper levels, per-block tail MAC), the second side stream (batch tiers) and the
+ * look-ahead stream of the block kernel.  Results must not change.  roles = 0 turns it off (the default): then nothing
+ * is added. */
+enum { DSPB200_STALL_MAIN = 1, DSPB200_STALL_SIDE = 2, DSPB200_STALL_SIDE2 = 4, DSPB200_STALL_HOT = 8 };
+int  dspb200_debug_stall(int roles, int microseconds, int period, int phase);
 
 /* ---- chain construction ---------------------------------------------------------------- */
 /* devices[n_devices]: CUDA ordinals to shard over (NULL/0: device 0).  slabs_per_device >= 1
