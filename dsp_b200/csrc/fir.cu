@@ -1326,19 +1326,16 @@ struct FirOp : Op {
 	long long *d_stats = nullptr;        // DSP_B200_FIR_PIPE_STATS: per-CTA cycle counters of the last pipeline launch
 	bool last_block_piped = false;
 	int batch_threads = getenv("DSP_B200_FIR_BATCH_THREADS") ? atoi(getenv("DSP_B200_FIR_BATCH_THREADS")) : 256;
-	cudaEvent_t ev_tail[2] = { nullptr, nullptr };
 	double *d_ring = nullptr, *d_ltmp = nullptr;
 	// side stream: the upper levels' partition-0 kernels and the last level's tail MAC overlap the main stream
 	cudaStream_t side = nullptr;
 	cudaEvent_t ev_main = nullptr, ev_urgent = nullptr;
-	// batch tiers: V spectra of the near tier (2 t_batch block periods) and of the far tier (2 t_far), on a second side stream
+	// batch tiers: V spectra of the near tier and of the far tier (FirSchedule::v_slots), on a second side stream
 	double2 *d_V = nullptr, *d_V2 = nullptr;
 	cudaStream_t side2 = nullptr;
-	cudaEvent_t ev_batch[2] = { nullptr, nullptr };
-	cudaEvent_t ev_bs[8] = {};           // after the tier launches of a block (ring), ev_bs_last: the latest one
-	int ev_bs_n = 0;
-	cudaEvent_t ev_bs_last = nullptr;
-	cudaEvent_t ev_bs_at[4] = {};        // folded: ev_bs_at[q & 3] = ev_bs_last as it was after block q
+	// the tail's event rings and what they hold (fir_tail_steps)
+	cudaEvent_t ev_tail[FIR_N_EV_TAIL] = {}, ev_batch[FIR_N_EV_BATCH] = {}, ev_bs[FIR_N_EV_BS] = {};
+	FirTailRing ring;
 	cudaEvent_t ev_join[2] = { nullptr, nullptr };
 	cudaStream_t hot = nullptr;          // FirSchedule::hot
 	cudaEvent_t ev_hot_in = nullptr, ev_hot_out = nullptr;
@@ -1380,10 +1377,11 @@ struct FirOp : Op {
 	{
 		for (cudaStream_t *q : { &side, &side2, &hot })
 			if (*q) { cudaStreamSynchronize(*q); cudaStreamDestroy(*q); *q = nullptr; }
-		for (cudaEvent_t *e : { &ev_hot_in, &ev_hot_out, &ev_batch[0], &ev_batch[1], &ev_tail[0], &ev_tail[1], &ev_join[0], &ev_join[1], &ev_main, &ev_urgent })
+		for (cudaEvent_t *e : { &ev_hot_in, &ev_hot_out, &ev_join[0], &ev_join[1], &ev_main, &ev_urgent })
 			if (*e) { cudaEventDestroy(*e); *e = nullptr; }
-		for (cudaEvent_t &e : ev_bs) { if (e) cudaEventDestroy(e); e = nullptr; }
-		ev_bs_last = nullptr; ev_bs_n = 0; for (cudaEvent_t &e : ev_bs_at) e = nullptr;
+		auto destroy = [](auto &es) { for (cudaEvent_t &e : es) { if (e) cudaEventDestroy(e); e = nullptr; } };
+		destroy(ev_tail); destroy(ev_batch); destroy(ev_bs);
+		ring = {};
 		for (FirLevel &L : lv) { dev_free(L.fdl); dev_free(L.H); dev_free(L.carry); dev_free(L.pend); L = FirLevel(); }
 		dev_free(d_V); dev_free(d_V2); dev_free(d_Y_side); dev_free(d_hist); dev_free(d_ytmp); dev_free(d_pre); dev_free(d_h0);
 		dev_free(d_Y); dev_free(d_ring); dev_free(d_ltmp); dev_free(d_Ybulk); dev_free(d_lo); dev_free(d_hi); dev_free(d_stats);
@@ -1421,6 +1419,7 @@ struct FirOp : Op {
 		}
 		auto stream = [](cudaStream_t &q, int prio) { CUDA_TRY(cudaStreamCreateWithPriority(&q, cudaStreamNonBlocking, prio), return false); return true; };
 		auto events = [](std::initializer_list<cudaEvent_t *> es) { for (cudaEvent_t *e : es) CUDA_TRY(cudaEventCreateWithFlags(e, cudaEventDisableTiming), return false); return true; };
+		auto ring_events = [&](auto &es) { for (cudaEvent_t &e : es) if (!events({ &e })) return false; return true; };
 		const size_t rows = (size_t) n_sel * s.lv[s.n_levels - 1].B;
 		int lo = 0, hi = 0;
 		cudaDeviceGetStreamPriorityRange(&lo, &hi);
@@ -1433,15 +1432,14 @@ struct FirOp : Op {
 			if (!stream(side, side_prio) || !events({ &ev_main, &ev_urgent })) return -1;
 		}
 		if (s.hot && (!stream(hot, hi) || !events({ &ev_hot_in, &ev_hot_out }))) return -1;
-		if (s.t_batch > 0 && !(d_V = dev_alloc<double2>(2 * s.t_batch * rows))) return -1;
-		if (s.t_batch > 0 && !s.use_pipe && (!stream(side2, lo) || !events({ &ev_batch[0], &ev_batch[1] }))) return -1;
-		if (s.t_far > 0 && !(d_V2 = dev_alloc<double2>(2 * s.t_far * rows))) return -1;
-		if (s.t_batch > 0 && !s.use_pipe && s.tail_pf == 2)
-			for (cudaEvent_t &e : ev_bs) if (!events({ &e })) return -1;
+		if (s.t_batch > 0 && !(d_V = dev_alloc<double2>(s.v_slots(0) * rows))) return -1;
+		if (s.t_batch > 0 && !s.use_pipe && (!stream(side2, lo) || !ring_events(ev_batch))) return -1;
+		if (s.t_far > 0 && !(d_V2 = dev_alloc<double2>(s.v_slots(1) * rows))) return -1;
+		if (s.t_batch > 0 && !s.use_pipe && s.tail_pf == 2 && !ring_events(ev_bs)) return -1;
 		if (s.use_pipe && k.pipe_stats) d_stats = dev_alloc<long long>(8 * 1024);
 		if (s.tail_pf > 0 && !s.use_pipe && !s.fold) {
-			if (!(d_Y_side = dev_alloc<double2>(s.tail_pf * rows))) return -1;
-			if (s.tail_pf == 2 && !events({ &ev_tail[0], &ev_tail[1] })) return -1;
+			if (!(d_Y_side = dev_alloc<double2>(s.y_slots() * rows))) return -1;
+			if (s.tail_pf == 2 && !ring_events(ev_tail)) return -1;
 		}
 		const int B0 = s.B0;
 		if (s.nb_max > 1) {
@@ -1514,10 +1512,9 @@ struct FirOp : Op {
 		if (!planned) return;
 		if (side) cudaStreamSynchronize(side);
 		if (side2) cudaStreamSynchronize(side2);
-		if (d_V) cudaMemsetAsync(d_V, 0, (size_t) 2 * s.t_batch * n_sel * s.lv[s.n_levels - 1].B * sizeof(double2), st);
-		if (d_V2) cudaMemsetAsync(d_V2, 0, (size_t) 2 * s.t_far * n_sel * s.lv[s.n_levels - 1].B * sizeof(double2), st);
-		ev_bs_last = nullptr;
-		for (cudaEvent_t &e : ev_bs_at) e = nullptr;
+		if (d_V) cudaMemsetAsync(d_V, 0, (size_t) s.v_slots(0) * n_sel * s.lv[s.n_levels - 1].B * sizeof(double2), st);
+		if (d_V2) cudaMemsetAsync(d_V2, 0, (size_t) s.v_slots(1) * n_sel * s.lv[s.n_levels - 1].B * sizeof(double2), st);
+		ring = {};
 		for (int l = 0; l < s.n_levels; ++l) {
 			FirLevel &L = lv[l];
 			const FirLevelPlan &Lp = s.lv[l];
@@ -1575,7 +1572,7 @@ struct FirOp : Op {
 		// held up, and in device-resident mode it is faster too than with the partition-0 kernels on the caller's
 		// stream: the caller's stream keeps only stash, level 0, unstash.
 		const bool serial = g_fir_serialize.load(std::memory_order_relaxed) != 0;
-		cudaStream_t us = serial ? st : side, ts = us, bs = serial ? st : side2;
+		cudaStream_t us = serial ? st : side;
 		bool any = false;
 		for (int l = 1; l < s.n_levels; ++l) {
 			FirLevel &L = lv[l];
@@ -1600,24 +1597,64 @@ struct FirOp : Op {
 		if (!any) return 0;
 		CUDA_TRY(cudaEventRecord(ev_urgent, us), return -1);
 		urgent_pending = (us != st);
-		const int lt = s.n_levels - 1;
-		const FirLevel &L = lv[lt]; const FirLevelPlan &Lp = s.lv[lt];
-		if (Lp.tail && s.tail_pf == 1 && abs_pos % Lp.B == 0) {
-			const long q1 = L.blk;   // Y_{q+1} = MAC + V_{q+1}, q = the block that just completed
-			const long qb = s.tier_wait(q1);
-			if (qb >= 0) CUDA_TRY(cudaStreamWaitEvent(ts, ev_batch[(qb / s.t_batch) & 1], 0), return -1);
-			const double2 *init = (s.t_batch > 0) ? d_V + (size_t) (q1 % (2 * s.t_batch)) * n_sel * Lp.B : nullptr;
-			mac(lt, s.mac_parts().first, s.mac_parts().second, q1, ts, d_Y_side, init);
-			const long q = q1 - 1;
-			const FirTierLaunches tl = fir_tier_launches(s, q, n_sel);
-			if (tl.n > 0) {
-				// X_q is in the FDL once the partition-0 kernel of this block has run (ev_urgent on the side stream)
-				CUDA_TRY(cudaStreamWaitEvent(bs, ev_urgent, 0), return -1);
-				if (bs != st) stall_on(DSPB200_STALL_SIDE2, lv[0].blk - 1, bs);
-				const int threads = (Lp.B < batch_threads_for(s.t_batch)) ? Lp.B : batch_threads_for(s.t_batch);
-				launch_mac_batch(s.t_batch, fc == 1, dim3(Lp.B / threads, n_sel), threads, bs, batch_args(tl.l[0], q));
-				CUDA_TRY(cudaEventRecord(ev_batch[(q / s.t_batch) & 1], bs), return -1);
+		if (abs_pos % s.Bmax != 0) return 0;   // the last level's block is not complete
+		return launch_tail(lv[s.n_levels - 1].blk - 1, st, us, serial ? st : side2);
+	}
+
+	// the event of a FirEv (FirEvRing order), and slot i of a ring of spectra of the tail level (FirSchedule::v_slots)
+	cudaEvent_t event(const FirEv &e) const
+	{
+		const cudaEvent_t *rings[] = { nullptr, &ev_main, &ev_urgent, ev_tail, ev_batch, ev_bs };
+		return rings[e.ring][e.slot];
+	}
+	double2 *slot(double2 *spectra, int i) const { return spectra + (size_t) i * n_sel * s.lv[s.n_levels - 1].B; }
+	int wait(cudaStream_t st, const FirEv &e)
+	{
+		if (e.ring != FIR_EV_NONE) CUDA_TRY(cudaStreamWaitEvent(st, event(e), 0), return -1);
+		return 0;
+	}
+
+	// The launches after block q of the tail level (fir_tail_steps), the side roles on ts and bs; either may be the caller's
+	// stream st, which then has no ev_main to wait for.  The stall hook delays a side stream where it starts on the block.
+	int launch_tail(long q, cudaStream_t st, cudaStream_t ts, cudaStream_t bs)
+	{
+		const FirLevel &L = lv[s.n_levels - 1];
+		const FirLevelPlan &Lp = s.lv[s.n_levels - 1];
+		const FirTailSteps steps = fir_tail_steps(s, q, n_sel, ring);
+		for (int i = 0; i < steps.n; ++i) {
+			const FirTailStep &x = steps.l[i];
+			cudaStream_t xs = (x.role == FIR_SIDE2) ? bs : ts;
+			for (const FirEv &w : x.wait)
+				if (!(w.ring == FIR_EV_MAIN && xs == st) && wait(xs, w)) return -1;
+			if ((x.wait[0].ring == FIR_EV_MAIN || x.wait[0].ring == FIR_EV_URGENT) && xs != st)
+				stall_on((x.role == FIR_SIDE2) ? DSPB200_STALL_SIDE2 : DSPB200_STALL_SIDE, lv[0].blk - 1, xs);
+			double2 *Y = (x.kind != FIR_TAIL_TIER) ? slot(d_Y_side, x.y) : nullptr;
+			const double2 *V = (x.v >= 0) ? slot(d_V, x.v) : nullptr;
+			if (x.kind == FIR_TAIL_MAC) mac(s.n_levels - 1, s.mac_parts().first, s.mac_parts().second, x.j, xs, Y, V);
+			else if (x.kind == FIR_TAIL_TIER) {
+				int threads = batch_threads_for(x.d.T);
+				if (s.n_levels == 1 && (batch_threads == 128 || batch_threads == 64) && batch_threads < threads) threads = batch_threads;
+				if (Lp.B < threads) threads = Lp.B;
+				// whole launches of the far tier: at most one CTA per SM (DSP_B200_FIR_FAR_SMEM_KB, 0 = no cap)
+				static const long far_kb = getenv("DSP_B200_FIR_FAR_SMEM_KB") ? atol(getenv("DSP_B200_FIR_FAR_SMEM_KB")) : 0;
+				launch_mac_batch(x.d.T, fc == 1, dim3(Lp.B / threads, x.d.rows + x.d.pass_rows), threads, xs, batch_args(x.d, q),
+				                 x.d.tier ? "fir_mac_batch_far" : "fir_mac_batch", (x.d.tier && !s.stagger && far_kb > 0) ? (size_t) far_kb * 1024 : 0);
 			}
+			else {
+				// one grid for the per-block MAC and this block's class of the near tier
+				TailArgs ta = {};
+				ta.m.fdl = L.fdl; ta.m.H = L.H; ta.m.Y = Y; ta.m.init = V;
+				ta.m.N = Lp.B; ta.m.P = Lp.R; ta.m.slot0 = (int) (x.j % Lp.R); ta.m.p0 = s.mac_parts().first; ta.m.p1 = s.mac_parts().second;
+				ta.m.h_ch_stride = (fc == 1) ? 0 : (long) Lp.P * Lp.B;
+				ta.b = batch_args(x.d, q);
+				ta.n_batch_y = x.d.rows;
+				const dim3 grid(Lp.B / 256, ta.n_batch_y + n_sel);
+				ProfScope prof("fir_tail", xs);
+				if (fc == 1) LAUNCH((k_fir_tail<4, true>), grid, 256, 0, xs, ta);
+				else LAUNCH((k_fir_tail<4, false>), grid, 256, 0, xs, ta);
+			}
+			for (const FirEv &e : x.rec)
+				if (e.ring != FIR_EV_NONE) CUDA_TRY(cudaEventRecord(event(e), xs), return -1);
 		}
 		return 0;
 	}
@@ -1629,10 +1666,10 @@ struct FirOp : Op {
 		const FirLevelPlan &Lp = s.lv[s.n_levels - 1];
 		MacBatchArgs b = {};
 		b.fdl = L.fdl; b.H = L.H; b.N = Lp.B; b.P = Lp.P; b.n_sel = n_sel; b.q = q;
-		b.V = d.tier ? d_V2 : d_V; b.n_slots = 2 * d.T;
+		b.V = d.tier ? d_V2 : d_V; b.n_slots = s.v_slots(d.tier);
 		b.h_ch_stride = (fc == 1) ? 0 : (long) Lp.P * Lp.B;
 		b.pf = d.pf; b.p_lo = d.p_lo; b.p_hi = d.p_hi; b.g = d.g; b.K = d.K; b.w = d.w;
-		if (d.from_far) { b.Vin = d_V2; b.vin_slots = 2 * s.t_far; }
+		if (d.from_far) { b.Vin = d_V2; b.vin_slots = s.v_slots(1); }
 		if (d.pass_rows > 0) { b.n_tier_y = d.rows; b.pass_g = d.pass_g; b.pass_m = d.pass_m; }
 		return b;
 	}
@@ -1650,9 +1687,7 @@ struct FirOp : Op {
 		// the MAC queued behind the fused kernel on the caller's stream, where it runs alone -- DSP_B200_FIR_TAIL_MAIN=1
 		// selects that for measurements).
 		static const int tail_main = getenv("DSP_B200_FIR_TAIL_MAIN") ? atoi(getenv("DSP_B200_FIR_TAIL_MAIN")) : -1;
-		const bool on_main = serial || tail_main > 0;
-		cudaStream_t ts = on_main ? st : side, bs = serial ? st : side2;
-		const long q = L.blk - 1, j = q + 2;
+		const long q = L.blk - 1;
 		if (s.use_pipe) {
 			// The pipeline kernel of block q does block q's share of the batched tail itself (channels of residue
 			// q % 4: V_{q+2} .. V_{q+5} from the blocks up to q-1).  A block that took the general path gets the same
@@ -1667,85 +1702,8 @@ struct FirOp : Op {
 			}
 			return 0;
 		}
-		if (s.fold) {
-			if (!serial) CUDA_TRY(cudaEventRecord(ev_main, st), return -1);
-			if (launch_tiers0(q, bs, serial)) return -1;
-			ev_bs_at[q & 3] = ev_bs_last;
-			return 0;
-		}
-		double2 *Y = d_Y_side + (size_t) (j & 1) * n_sel * Lp.B;
-		if (!serial) {
-			CUDA_TRY(cudaEventRecord(ev_main, st), return -1);
-			if (!on_main) CUDA_TRY(cudaStreamWaitEvent(side, ev_main, 0), return -1);
-		}
-		if (s.merge_tail) {
-			// one grid for the per-block MAC (Y_{q+2}) and this block's class of the batch tier
-			TailArgs ta = {};
-			ta.m.fdl = L.fdl; ta.m.H = L.H; ta.m.Y = Y; ta.m.init = d_V + (size_t) (j % (2 * s.t_batch)) * n_sel * Lp.B;
-			ta.m.N = Lp.B; ta.m.P = Lp.R; ta.m.slot0 = (int) (j % Lp.R); ta.m.p0 = s.mac_parts().first; ta.m.p1 = s.mac_parts().second;
-			ta.m.h_ch_stride = (fc == 1) ? 0 : (long) Lp.P * Lp.B;
-			const FirTierLaunches tl = fir_tier_launches(s, q, n_sel);
-			ta.b = batch_args(tl.l[0], q);
-			ta.n_batch_y = tl.l[0].rows;
-			const dim3 grid(Lp.B / 256, ta.n_batch_y + n_sel);
-			if (!on_main) stall_on(DSPB200_STALL_SIDE, q, ts);
-			{
-				ProfScope prof("fir_tail", ts);
-				if (fc == 1) LAUNCH((k_fir_tail<4, true>), grid, 256, 0, ts, ta);
-				else LAUNCH((k_fir_tail<4, false>), grid, 256, 0, ts, ta);
-			}
-			CUDA_TRY(cudaEventRecord(ev_tail[j & 1], ts), return -1);
-			cudaEvent_t e = ev_bs[ev_bs_n++ & 7];   // the general path waits for the batch part through this one
-			CUDA_TRY(cudaEventRecord(e, ts), return -1);
-			ev_bs_last = e;
-			return 0;
-		}
-		// the tier launches up to block q-1 = tier_wait(j): every one made so far
-		if (s.t_batch > 0 && ev_bs_last) CUDA_TRY(cudaStreamWaitEvent(ts, ev_bs_last, 0), return -1);
-		if (!on_main) stall_on(DSPB200_STALL_SIDE, q, ts);
-		mac(0, s.mac_parts().first, s.mac_parts().second, j, ts, Y, (s.t_batch > 0) ? d_V + (size_t) (j % (2 * s.t_batch)) * n_sel * Lp.B : nullptr);
-		CUDA_TRY(cudaEventRecord(ev_tail[j & 1], ts), return -1);
-		if (s.t_batch > 0 && launch_tiers0(q, bs, serial)) return -1;
-		return 0;
-	}
-
-	// the tier launches after block q of a single-level plan (fir_tier_launches)
-	int launch_tiers0(long q, cudaStream_t bs, bool serial)
-	{
-		const FirTierLaunches tl = fir_tier_launches(s, q, n_sel);
-		bool any = false;
-		for (int i = 0; i < tl.n; ++i) {
-			const FirTierLaunch &d = tl.l[i];
-			if (d.rows + d.pass_rows == 0) continue;
-			if (!any && !serial) {
-				CUDA_TRY(cudaStreamWaitEvent(bs, ev_main, 0), return -1);
-				stall_on(DSPB200_STALL_SIDE2, q, bs);
-			}
-			any = true;
-			int threads = batch_threads_for(d.T);
-			if ((batch_threads == 128 || batch_threads == 64) && batch_threads < threads) threads = batch_threads;
-			if (s.B0 < threads) threads = s.B0;
-			// whole launches of the far tier: at most one CTA per SM (DSP_B200_FIR_FAR_SMEM_KB, 0 = no cap)
-			static const long far_kb = getenv("DSP_B200_FIR_FAR_SMEM_KB") ? atol(getenv("DSP_B200_FIR_FAR_SMEM_KB")) : 0;
-			launch_mac_batch(d.T, fc == 1, dim3(s.B0 / threads, d.rows + d.pass_rows), threads, bs, batch_args(d, q),
-			                 d.tier ? "fir_mac_batch_far" : "fir_mac_batch", (d.tier && !s.stagger && far_kb > 0) ? (size_t) far_kb * 1024 : 0);
-		}
-		if (any) {
-			cudaEvent_t e = ev_bs[ev_bs_n++ & 7];
-			CUDA_TRY(cudaEventRecord(e, bs), return -1);
-			ev_bs_last = e;
-		}
-		return 0;
-	}
-
-	// the general path's block of a single-level tail plan waits for every tier launch made so far (FirSchedule::tier_wait
-	// is what the fused kernel's path waits for)
-	int wait_batch_for(long blk, cudaStream_t st)
-	{
-		(void) blk;
-		if (s.t_batch > 0 && s.tail_pf == 2 && !s.use_pipe && ev_bs_last && !g_fir_serialize.load(std::memory_order_relaxed))
-			CUDA_TRY(cudaStreamWaitEvent(st, ev_bs_last, 0), return -1);
-		return 0;
+		if (!serial) CUDA_TRY(cudaEventRecord(ev_main, st), return -1);
+		return launch_tail(q, st, (serial || tail_main > 0) ? st : side, serial ? st : side2);
 	}
 
 	// What the unstash / head kernels add on top of level 0 for the frames starting at `first_frame_abs`:
@@ -1954,7 +1912,7 @@ struct FirOp : Op {
 					f.fdl = L0.fdl; f.fdl_ch_stride = (long) Lp0.R * s.B0; f.fdl_rows = Lp0.R; f.slot = (int) (L0.blk % Lp0.R);
 					f.H = L0.H; f.h_ch_stride = (fc == 1) ? 0 : (long) Lp0.P * s.B0;
 					f.P = Lp0.P; f.pf = s.pipe_pf;
-					f.V = (s.t_batch > 0) ? d_V : nullptr; f.v_slots = 2 * s.t_batch; f.blk = L0.blk;
+					f.V = (s.t_batch > 0) ? d_V : nullptr; f.v_slots = s.v_slots(0); f.blk = L0.blk;
 					f.carry = L0.carry; f.tw = L0.tw; f.ptw = L0.ptw; f.n_ch = n_sel;
 					f.evict_first = pipe_evict_first;
 					f.fake_io = (pipe_fake_io && C == n_sel && dstride == C) ? 1 : 0;
@@ -1993,19 +1951,13 @@ struct FirOp : Op {
 						CUDA_TRY(cudaStreamWaitEvent(hot, ev_hot_in, 0), return -1);
 						ls = hot;
 					}
+					const FirTailRead c = fir_fused_read(s, L0.blk, ring);
+					if (wait(ls, c.wait)) return -1;
+					if (c.v >= 0) f.init = slot(d_V, c.v);
+					if (c.y >= 0) f.init = slot(d_Y_side, c.y);
 					if (s.fold) {
-						// (before any launch has covered V_j it is zero: the blocks it sums do not exist)
-						if (const long qw = s.tier_wait(L0.blk); qw >= 0) {
-							if (cudaEvent_t e = ev_bs_at[qw & 3]) CUDA_TRY(cudaStreamWaitEvent(ls, e, 0), return -1);
-							f.init = d_V + (size_t) (L0.blk % (2 * s.t_batch)) * n_sel * s.B0;
-						}
 						f.blk = L0.blk;
 						f.cls_T = s.t_batch; f.cls_K = s.stagger ? s.t_batch : 1; f.cls_w = s.class_w; f.la = s.la; f.pass_m = s.pass_m;
-					}
-					else if (s.tail_pf == 2 && L0.blk >= 2) {
-						// Y of this block was launched two blocks ago (advance_tail0)
-						CUDA_TRY(cudaStreamWaitEvent(ls, ev_tail[L0.blk & 1], 0), return -1);
-						f.init = d_Y_side + (size_t) (L0.blk & 1) * n_sel * s.B0;
 					}
 					if (use_hot) stall_on(DSPB200_STALL_HOT, L0.blk, hot);
 					if (launch_level0(s.B0, f, ls)) return -1;
@@ -2037,7 +1989,7 @@ struct FirOp : Op {
 				if (pos + seg == s.B0) {
 					// block complete: X into the FDL, carry = IRFFT(S)[B:2B) (its first half has been emitted already)
 					last_block_piped = false;
-					if (wait_batch_for(L0.blk, st)) return -1;
+					if (!g_fir_serialize.load(std::memory_order_relaxed) && wait(st, fir_general_wait(L0.blk, ring))) return -1;
 					if (level_block(0, nullptr, 0, INV_UPDATE_CARRY, st)) return -1;
 					++n_general;
 					pre_valid = false;

@@ -138,6 +138,11 @@ struct FirSchedule {
 		if (n_levels > 1) return (j >= 2) ? t_batch * ((j - 2) / t_batch) : -1;
 		return j - (fold ? la : merge_tail ? 2 : 3);
 	}
+	// Slots of the tail level's spectrum rings: V of the near (tier 0) or far tier (1), Y; and the slot of period j
+	int v_slots(int tier) const { return 2 * (tier ? t_far : t_batch); }
+	int y_slots() const { return tail_pf; }
+	int v_slot(long j) const { return (int) (j % v_slots(0)); }
+	int y_slot(long j) const { return (int) (j % y_slots()); }
 };
 
 #ifdef __CUDA_ARCH__
@@ -315,6 +320,76 @@ inline FirTierLaunches fir_tier_launches(const FirSchedule &s, long q, int n_sel
 	}
 	return r;
 }
+
+// ---- The tail's cross-stream protocol; fir.cu maps its stream roles to streams and its slots to events and spectra.
+enum FirEvRing { FIR_EV_NONE, FIR_EV_MAIN, FIR_EV_URGENT, FIR_EV_TAIL, FIR_EV_BATCH, FIR_EV_BS };
+constexpr int FIR_N_EV_TAIL = 2, FIR_N_EV_BATCH = 2, FIR_N_EV_BS = 8, FIR_N_BS_AT = 4;
+// ev_main / ev_urgent: the caller stream after block q / the side stream after the upper level's partition-0 kernels.
+// blk: a label for tests/test_fir_tiers_cpu.py (fir.cu does not read it), the block (ev_tail: period) the event marks.
+struct FirEv { int ring = FIR_EV_NONE, slot = 0; long blk = 0; };
+// ev_bs records so far (record n >= 1 in slot (n - 1) mod FIR_N_EV_BS); folded, at[q mod FIR_N_BS_AT]: n after block q
+struct FirTailRing { long n = 0; long at[FIR_N_BS_AT] = {}; };
+inline int fir_bs_slot(long n) { return (int) ((n - 1) % FIR_N_EV_BS); }
+
+enum FirTailKind { FIR_TAIL_MAC, FIR_TAIL_MERGED, FIR_TAIL_TIER };
+enum FirTailRole { FIR_SIDE, FIR_SIDE2 };
+struct FirTailStep {
+	int kind = FIR_TAIL_MAC, role = FIR_SIDE;
+	FirEv wait[2], rec[2];   // waited for before it (ev_main, ev_urgent first), recorded after it
+	long j = 0;              // MAC, merged grid: Y_j into Y slot y, from V slot v (-1: zero)
+	int y = -1, v = -1;
+	FirTierLaunch d = {};    // tier launch; the merged grid's batch rows
+};
+struct FirTailSteps { int n = 0; FirTailStep l[3]; };
+
+// The launches after block q of the tail level in issue order: unless folded, the per-block MAC of period q + tail_pf or
+// the merged grid (side stream), then the tier launches that have rows (second side stream).
+inline FirTailSteps fir_tail_steps(const FirSchedule &s, long q, int n_sel, FirTailRing &r)
+{
+	FirTailSteps o;
+	if (s.tail_pf == 0 || s.use_pipe) return o;
+	const bool l0 = s.tail_pf == 2;
+	const long j = q + s.tail_pf, qw = s.tier_wait(j);
+	const FirEv start = { l0 ? FIR_EV_MAIN : FIR_EV_URGENT, 0, q };
+	auto batch = [&](long b) { return FirEv{ FIR_EV_BATCH, (int) ((b / s.t_batch) % FIR_N_EV_BATCH), b }; };
+	auto bs_record = [&] { return FirEv{ FIR_EV_BS, (int) (r.n++ % FIR_N_EV_BS), q }; };
+	const FirTierLaunches tl = fir_tier_launches(s, q, n_sel);
+	if (!s.fold) {
+		FirTailStep &m = o.l[o.n++];
+		m.kind = s.merge_tail ? FIR_TAIL_MERGED : FIR_TAIL_MAC;
+		m.j = j; m.y = s.y_slot(j); m.v = (s.t_batch > 0) ? s.v_slot(j) : -1;
+		m.wait[0] = l0 ? start : (qw >= 0) ? batch(qw) : FirEv{};
+		if (l0 && !s.merge_tail && r.n > 0) m.wait[1] = { FIR_EV_BS, fir_bs_slot(r.n), qw };
+		if (l0) m.rec[0] = { FIR_EV_TAIL, (int) (j % FIR_N_EV_TAIL), j };
+		if (s.merge_tail) { m.d = tl.l[0]; m.rec[1] = bs_record(); return o; }
+	}
+	const int first = o.n;   // the tier launches that have rows: the first waits for the block, the last records
+	for (int i = 0; i < tl.n; ++i) {
+		if (tl.l[i].rows + tl.l[i].pass_rows == 0) continue;
+		FirTailStep &b = o.l[o.n++];
+		b.kind = FIR_TAIL_TIER; b.role = FIR_SIDE2; b.d = tl.l[i];
+	}
+	if (o.n > first) { o.l[first].wait[0] = start; o.l[o.n - 1].rec[0] = l0 ? bs_record() : batch(q); }
+	if (s.fold) r.at[q % FIR_N_BS_AT] = r.n;
+	return o;
+}
+
+// What the fused kernel of block j (single level) waits for and starts from (-1: zero, as V_j before block tier_wait(j))
+struct FirTailRead { FirEv wait; int y = -1, v = -1; };
+inline FirTailRead fir_fused_read(const FirSchedule &s, long j, const FirTailRing &r)
+{
+	FirTailRead c;
+	const long qw = s.tier_wait(j);
+	if (s.fold && qw >= 0) {
+		const long n = r.at[qw % FIR_N_BS_AT];
+		c.v = s.v_slot(j);
+		if (n > 0) c.wait = { FIR_EV_BS, fir_bs_slot(n), qw };
+	}
+	if (!s.fold && s.tail_pf == 2 && !s.use_pipe && j >= 2) { c.y = s.y_slot(j); c.wait = { FIR_EV_TAIL, (int) (j % FIR_N_EV_TAIL), j }; }
+	return c;
+}
+// The general path's block j (single level) overwrites an FDL row the tier launches read: after every one so far
+inline FirEv fir_general_wait(long j, const FirTailRing &r) { return (r.n > 0) ? FirEv{ FIR_EV_BS, fir_bs_slot(r.n), j - 1 } : FirEv{}; }
 
 // the schedule's part of FirOp::describe()
 inline std::string fir_schedule_json(const FirSchedule &s)

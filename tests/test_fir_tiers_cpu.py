@@ -1,10 +1,9 @@
 """CPU tier: the FIR tail schedule of dsp_b200/csrc/fir_plan.h, compiled with g++ alone.
 
-For every plan with a tail (the pipeline kernel's aside) the whole-block schedule is enumerated from the header's
-functions alone -- fir_tier_launches(), fir_batch_window(), fir_class_channel(), fir_fused_parts(),
-FirSchedule::mac_parts() and FirSchedule::tier_wait() -- as the launches fir.cu makes: the fused kernel of every block
-(one stream, in order), the per-block MAC or the merged grid (a side stream), the tier launches (a second side stream),
-over enough blocks to pass start-up and wrap the V and FDL rings several times.  Then:
+For every plan with a tail (the pipeline kernel's aside) the whole-block schedule fir.cu runs is enumerated from the
+header alone (fir_tail_steps(), fir_fused_read() and the functions they use): the fused kernel of every block (one stream,
+in order), the per-block MAC or the merged grid (a side stream), the tier launches (a second side stream), over enough
+blocks to pass start-up and wrap the V and FDL rings several times.  Then:
 
 1. exactly once: every partition p <= j of every period j of every channel is summed by exactly one launch;
 2. causality: a launch after block q reads only blocks <= q;
@@ -13,8 +12,8 @@ over enough blocks to pass start-up and wrap the V and FDL rings several times. 
    lands in between, and every write is read (a reader that finds no write reads the zeros of an unwritten slot);
 5. event rings: the event each wait uses still marks the block it means when the wait is enqueued.
 
-"Ordered" follows from in-order streams, "a launch after block q starts after the fused kernel of block q" and the
-wait rule tier_wait().  Each check is shown to fail on a broken copy of the headline's records.
+"Ordered" follows from in-order streams, "ev_main and ev_urgent mark the fused kernel of their block" and "a wait on a
+ring slot orders after the last record into it".  Each check is shown to fail on a broken copy of the headline's records.
 """
 import copy
 import ctypes
@@ -32,48 +31,57 @@ DRIVER = r"""
 #include "fir_plan.h"
 using namespace dspb200;
 static FirSchedule g;
+static FirTailRing r;
 extern "C" void plan(long taps, long hint, int n_sel, int sm_count, int *o)
 {
 	g = fir_schedule({ taps, hint, n_sel, sm_count, true, true }, FirKnobs::from_env());
+	r = {};
 	const FirLevelPlan &L = g.lv[g.n_levels - 1];
 	const int v[] = { g.n_levels, L.P, L.R, g.tail_pf, g.t_batch, g.t_far, g.fold, g.stagger, g.merge_tail, g.use_pipe,
-	                  g.mac_parts().first, g.mac_parts().second };
-	for (int i = 0; i < 12; ++i) o[i] = v[i];
+	                  g.mac_parts().first, g.mac_parts().second, g.v_slots(0), g.v_slots(1), g.y_slots() };
+	for (int i = 0; i < 15; ++i) o[i] = v[i];
 }
-extern "C" int tier_launches(long q, int n_sel, int *o)   // 13 ints per launch
-{
-	const FirTierLaunches r = fir_tier_launches(g, q, n_sel);
-	for (int i = 0; i < r.n; ++i) {
-		const FirTierLaunch &d = r.l[i];
-		const int v[] = { d.tier, d.T, d.g, d.K, d.w, d.pf, d.p_lo, d.p_hi, d.rows, d.from_far, d.pass_g, d.pass_rows, d.pass_m };
-		for (int k = 0; k < 13; ++k) o[13 * i + k] = v[k];
-	}
-	return r.n;
-}
-extern "C" long tier_wait(long j) { return g.tier_wait(j); }
+extern "C" FirTailSteps tail_steps(long q, int n_sel) { return fir_tail_steps(g, q, n_sel, r); }
+extern "C" FirTailRead fused_read(long j) { return fir_fused_read(g, j, r); }
+extern "C" const int consts[] = { FIR_N_EV_BS, FIR_N_BS_AT, FIR_N_EV_BATCH, FIR_N_EV_TAIL, sizeof(FirTailSteps), sizeof(FirTailRead) };
 // as fir.cu's fused kernel gets it: K = T classes when staggered, else 1; at most l0_parts()
 extern "C" int fused_parts(long blk, int s)
 {
 	return fir_fused_parts(blk, s, g.t_batch, g.stagger ? g.t_batch : 1, g.class_w, g.la, g.pass_m, g.l0_parts());
 }
-extern "C" void batch_window(int pass, int T, int p_lo, int p_hi, int pass_m, int *o)
-{
-	const FirBatchWindow w = fir_batch_window(pass != 0, T, p_lo, p_hi, pass_m);
-	o[0] = w.x_hi; o[1] = w.h_hi; o[2] = w.n_t;
-}
+extern "C" FirBatchWindow batch_window(bool pass, int T, int p_lo, int p_hi, int pass_m) { return fir_batch_window(pass, T, p_lo, p_hi, pass_m); }
 extern "C" int class_channel(int g_, int K, int w, int y) { return fir_class_channel(g_, K, w, y); }
 """
-PLAN_KEYS = ("n_levels", "P", "R", "tail_pf", "t_batch", "t_far", "fold", "stagger", "merge", "pipe", "mac_lo", "mac_hi")
-LAUNCH_KEYS = ("tier", "T", "g", "K", "w", "pf", "p_lo", "p_hi", "rows", "from_far", "pass_g", "pass_rows", "pass_m")
-RINGS = dict(ev_bs=8, ev_bs_at=4, ev_batch=2, ev_tail=2)   # fir.cu's event rings
+PLAN_KEYS = ("n_levels", "P", "R", "tail_pf", "t_batch", "t_far", "fold", "stagger", "merge", "pipe", "mac_lo", "mac_hi",
+             "V_slots", "V2_slots", "Y_slots")
+EV = (None, "ev_main", "ev_urgent", "ev_tail", "ev_batch", "ev_bs")   # FirEvRing
+MAC, MERGED, TIER = range(3)                                          # FirTailKind
+RINGS = {}   # the header's event rings, read when it is compiled (lib)
+
+
+def _struct(*fields):   # the layout of one of fir_plan.h's structs
+    return type("S", (ctypes.Structure,), dict(_fields_=[f if isinstance(f, tuple) else (f, ctypes.c_int) for f in fields]))
+
+
+Ev = _struct("ring", "slot", ("blk", ctypes.c_long))
+TierLaunch = _struct("tier", "T", "g", "K", "w", "pf", "p_lo", "p_hi", "rows", ("from_far", ctypes.c_bool), "pass_g", "pass_rows",
+                     "pass_m")
+TailStep = _struct("kind", "role", ("wait", Ev * 2), ("rec", Ev * 2), ("j", ctypes.c_long), "y", "v", ("d", TierLaunch))
+TailSteps = _struct("n", ("l", TailStep * 3))
+TailRead = _struct(("wait", Ev), "y", "v")
+BatchWindow = _struct("x_hi", "h_hi", "n_t")
 
 
 @pytest.fixture(scope="module")
 def lib(tmp_path_factory):
     lib = header_lib(tmp_path_factory.mktemp("fir_tiers"), "firtiers", DRIVER)
-    lib.tier_wait.argtypes, lib.tier_wait.restype = [ctypes.c_long], ctypes.c_long
-    lib.tier_launches.argtypes = [ctypes.c_long, ctypes.c_int, ctypes.c_void_p]
+    lib.tail_steps.argtypes, lib.tail_steps.restype = [ctypes.c_long, ctypes.c_int], TailSteps
+    lib.fused_read.argtypes, lib.fused_read.restype = [ctypes.c_long], TailRead
     lib.fused_parts.argtypes = [ctypes.c_long, ctypes.c_int]
+    lib.batch_window.argtypes, lib.batch_window.restype = [ctypes.c_bool] + [ctypes.c_int] * 4, BatchWindow
+    o = list((ctypes.c_int * 6).in_dll(lib, "consts"))
+    RINGS.update(zip(("ev_bs", "ev_bs_at", "ev_batch", "ev_tail"), o))
+    assert o[4:] == [ctypes.sizeof(TailSteps), ctypes.sizeof(TailRead)]   # the header's layout
     return lib
 
 
@@ -106,7 +114,7 @@ class Schedule:
     """The whole-block schedule of one plan: launch records in issue order and the event operations between them."""
 
     def __init__(self, lib, taps, hint, C, envs):
-        o = (ctypes.c_int * 12)()
+        o = (ctypes.c_int * len(PLAN_KEYS))()
         with env(**{k: None for k in os.environ if k.startswith("DSP_B200_FIR_")}):
             with env(**envs):
                 lib.plan(ctypes.c_long(taps), ctypes.c_long(hint), C, SMS, o)
@@ -116,20 +124,27 @@ class Schedule:
         self.has_tail = p["tail_pf"] > 0 and not p["pipe"]
         self.P, self.R = p["P"], p["R"]
         self.Q = 3 * self.P + 4 * max(p["t_batch"], p["t_far"], 1) + 4
-        self.slots = dict(V=2 * p["t_batch"], V2=2 * p["t_far"], Y=p["tail_pf"])
+        self.slots = dict(V=p["V_slots"], V2=p["V2_slots"], Y=p["Y_slots"])
 
-    def launches(self, q):
-        buf = (ctypes.c_int * 26)()
-        n = self.lib.tier_launches(q, self.C, buf)
-        return [dict(zip(LAUNCH_KEYS, buf[13 * i:13 * i + 13])) for i in range(n)]
-
-    def window(self, pass_, d):
-        o = (ctypes.c_int * 3)()
-        self.lib.batch_window(int(pass_), d["T"], d["p_lo"], d["p_hi"], d["pass_m"], o)
-        return tuple(o)
-
-    def chans(self, g, K, w, rows):
-        return np.array([self.lib.class_channel(g, K, w, y) for y in range(rows)], dtype=np.int64)
+    def tier_parts(self, q, d, sums, reads, vacc):
+        """Add the sums, reads and vacc of the tier launch d after block q (and of the mid-window pass it runs)."""
+        for pass_, g, rows in ((False, d.g, d.rows), (True, d.pass_g, d.pass_rows)):
+            if rows == 0:
+                continue
+            ch = np.array([self.lib.class_channel(g, d.K, d.w, y) for y in range(rows)], dtype=np.int64)
+            w = self.lib.batch_window(pass_, d.T, d.p_lo, d.p_hi, d.pass_m)
+            x_hi, h_hi, n_t = w.x_hi, w.h_hi, w.n_t
+            pf = d.pf
+            reads.append((q + pf + 1 - (x_hi - 1), q))   # FDL rows m in [pf+1, x_hi): X_{q+pf+1-m}
+            for t in range(n_t):
+                j = q + pf + 1 + t
+                sums.append((ch, j, max(pf + 1 + t, d.p_lo), min(x_hi + t, h_hi)))
+                if pass_:
+                    vacc.append((ch, "V", j, "acc"))
+                else:
+                    vacc.append((ch, "V2" if d.tier else "V", j, "init"))
+                    if d.from_far:
+                        vacc.append((ch, "V2", j, "read"))
 
     def enumerate(self):
         """-> (records, ops).  A record is one launch: id, stream, kind, q (the block it follows; a fused kernel's own
@@ -139,94 +154,51 @@ class Schedule:
         p, lib, C = self.p, self.lib, self.C
         allc = np.arange(C)
         recs, ops = [], []
-        mac_of = {}                   # period -> the record that writes its Y
+        marks = {}                    # (ring, slot) -> the record last recorded into it
         tier_upto = []                # tier_upto[q]: the last tier record issued after a block <= q
-        bs_n, bs_last, bs_at = 0, None, [None] * RINGS["ev_bs_at"]
-        multi = p["tail_pf"] == 1
 
         def rec(stream, kind, q, waits, sums=(), reads=(), vacc=()):
             recs.append(dict(id=len(recs), stream=stream, kind=kind, q=q, waits=[w for w in waits if w is not None],
                              sums=list(sums), reads=list(reads), vacc=list(vacc)))
             return recs[-1]["id"]
 
-        def last_tier(qw):
-            return tier_upto[qw] if 0 <= qw < len(tier_upto) else None
-
-        def tier_parts(q):
-            """-> [(tier, sums, reads, vacc)] of the tier launches after block q that have rows"""
-            out = []
-            for d in self.launches(q):
-                sums, reads, vacc = [], [], []
-                for pass_, g, rows in ((False, d["g"], d["rows"]), (True, d["pass_g"], d["pass_rows"])):
-                    if rows == 0:
-                        continue
-                    ch = self.chans(g, d["K"], d["w"], rows)
-                    x_hi, h_hi, n_t = self.window(pass_, d)
-                    pf = d["pf"]
-                    reads.append((q + pf + 1 - (x_hi - 1), q))   # FDL rows m in [pf+1, x_hi): X_{q+pf+1-m}
-                    for t in range(n_t):
-                        j = q + pf + 1 + t
-                        sums.append((ch, j, max(pf + 1 + t, d["p_lo"]), min(x_hi + t, h_hi)))
-                        if pass_:
-                            vacc.append((ch, "V", j, "acc"))
-                        else:
-                            vacc.append((ch, "V2" if d["tier"] else "V", j, "init"))
-                            if d["from_far"]:
-                                vacc.append((ch, "V2", j, "read"))
-                if sums:
-                    out.append((d["tier"], sums, reads, vacc))
-            return out
+        def wait(ev, F):
+            """-> the record a wait orders after; a ring slot's wait is checked to still mark the block it means"""
+            ring = EV[ev.ring]
+            if ring in ("ev_main", "ev_urgent"):
+                return F
+            ops.append(("wait", ring, ev.slot, recs[tier_upto[ev.blk]]["q"] if ring == "ev_bs" else ev.blk))
+            return marks.get((ring, ev.slot))
 
         for q in range(self.Q):
             # the fused kernel of block q (upper level: on the side stream, in order with the MAC)
-            if multi:
+            if p["tail_pf"] == 1:
                 F = rec("M", "fused", q, [], [(allc, q, 0, p["mac_lo"])], (), [(allc, "Y", q, "read")] if q >= 1 else [])
-            elif p["fold"]:
-                qw = lib.tier_wait(q)
-                nps = np.array([lib.fused_parts(q, s) for s in range(C)])
-                if qw >= 0:
-                    ops.append(("wait", "ev_bs_at", qw % RINGS["ev_bs_at"], qw))
-                    if bs_at[qw % RINGS["ev_bs_at"]] is not None:
-                        ops.append(("wait", "ev_bs", bs_at[qw % RINGS["ev_bs_at"]], recs[last_tier(qw)]["q"]))
-                F = rec("F", "fused", q, [last_tier(qw)], [(allc, q, 0, nps)], (), [(allc, "V", q, "read")] if qw >= 0 else [])
             else:
-                if q >= 2:
-                    ops.append(("wait", "ev_tail", q % RINGS["ev_tail"], q))
-                F = rec("F", "fused", q, [mac_of.get(q)], [(allc, q, 0, p["mac_lo"])], (), [(allc, "Y", q, "read")] if q >= 2 else [])
+                c = lib.fused_read(q)
+                nps = np.array([lib.fused_parts(q, s) for s in range(C)]) if p["fold"] else p["mac_lo"]
+                vacc = [(allc, b, q, "read") for b, i in (("V", c.v), ("Y", c.y)) if i >= 0]
+                F = rec("F", "fused", q, [wait(c.wait, None)] if c.wait.ring else [], [(allc, q, 0, nps)], (), vacc)
 
-            # what follows block q: the per-block MAC of period q + tail_pf, the tier launches after block q
-            j = q + p["tail_pf"]
-            mac = ([(allc, j, p["mac_lo"], p["mac_hi"])], [(j - p["mac_hi"] + 1, j - p["mac_lo"])],
-                   [(allc, "Y", j, "init")] + ([(allc, "V", j, "read")] if p["t_batch"] else []))
+            # what follows block q: the per-block MAC of period q + tail_pf or the merged grid, the tier launches
+            steps = lib.tail_steps(q, C)
             made = []
-            if p["merge"]:
-                parts = tier_parts(q)
-                sums, reads, vacc = (list(x) for x in mac)
-                for _, s_, r_, v_ in parts:
-                    sums += s_; reads += r_; vacc += v_
-                mac_of[j] = rec("M", "merged", q, [F], sums, reads, vacc)
-                made = [mac_of[j]]
-            else:
-                if not p["fold"]:
-                    qw = lib.tier_wait(j)
-                    if multi and qw >= 0:
-                        ops.append(("wait", "ev_batch", (qw // p["t_batch"]) % RINGS["ev_batch"], qw))
-                    if not multi and bs_last is not None:
-                        ops.append(("wait", "ev_bs", bs_last, recs[last_tier(qw)]["q"]))
-                    mac_of[j] = rec("M", "mac", q, [F, last_tier(qw)], *mac)
-                for tier, s_, r_, v_ in tier_parts(q):
-                    made.append(rec("B", "far" if tier else "near", q, [F], s_, r_, v_))
-                if multi and made:
-                    ops.append(("rec", "ev_batch", (q // p["t_batch"]) % RINGS["ev_batch"], q))
-            if not multi and not p["fold"]:
-                ops.append(("rec", "ev_tail", j % RINGS["ev_tail"], j))
-            if made and not multi:
-                bs_last = bs_n % RINGS["ev_bs"]
-                bs_n += 1
-                ops.append(("rec", "ev_bs", bs_last, q))
-            if p["fold"]:
-                bs_at[q % RINGS["ev_bs_at"]] = bs_last
-                ops.append(("rec", "ev_bs_at", q % RINGS["ev_bs_at"], q))
+            for x in steps.l[:steps.n]:
+                sums, reads, vacc = [], [], []
+                if x.kind != TIER:
+                    sums.append((allc, x.j, p["mac_lo"], p["mac_hi"]))
+                    reads.append((x.j - p["mac_hi"] + 1, x.j - p["mac_lo"]))
+                    vacc += [(allc, b, x.j, m) for b, i, m in (("Y", x.y, "init"), ("V", x.v, "read")) if i >= 0]
+                if x.kind != MAC:
+                    self.tier_parts(q, x.d, sums, reads, vacc)
+                kind = ("mac", "merged", "far" if x.d.tier else "near")[x.kind]
+                r = rec(("M", "B")[x.role], kind, q, [wait(w, F) for w in x.wait if w.ring], sums, reads, vacc)
+                if x.kind != MAC:
+                    made.append(r)
+                for e in x.rec:
+                    if e.ring:
+                        marks[(EV[e.ring], e.slot)] = r
+                        ops.append(("rec", EV[e.ring], e.slot, e.blk))
             tier_upto.append(made[-1] if made else (tier_upto[-1] if tier_upto else None))
         return recs, ops
 

@@ -74,7 +74,7 @@ def stalled(gpu_lib, roles, us, period=1, phase=0):
 
 
 def _roles(plan, device):
-    """The streams a plan enqueues FIR launches on (fir.cu: advance_upper_levels, advance_tail0, launch_tiers0, run)."""
+    """The streams a plan enqueues FIR launches on (fir.cu: advance_upper_levels, advance_tail0, launch_tail, run)."""
     multi = len(plan["levels"]) > 1
     tail0 = not multi and plan["tail_pf"] == 2 and not plan["pipe"]
     fold = tail0 and plan["l0_parts"] > 2
