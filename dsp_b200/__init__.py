@@ -6,4 +6,4 @@ Python package is the thin binding used by tests and bench.py; it has no CPU pat
 """
 from .lib import (Chain, DspB200Error, debug_serialize, debug_stall, PinnedArray, biquad_design, device_count, hilbert_taps,  # noqa: F401
                   kernel_launches, last_error, lib, profile_enable, profile_read, resample_params, copy_counts,
-                  STALL_HOT, STALL_MAIN, STALL_SIDE, STALL_SIDE2)
+                  STALL_HOT, STALL_MAIN, STALL_SIDE, STALL_SIDE2, IO_F32, IO_F64, IO_PLANAR, io_format)

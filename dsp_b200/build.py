@@ -10,7 +10,7 @@ import sys
 
 HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
-SOURCES = ["api.cu", "fir.cu", "biquad.cu", "resample.cu", "design.cu", "delay.cu"]
+SOURCES = ["api.cu", "fir.cu", "biquad.cu", "resample.cu", "design.cu", "delay.cu", "edge.cu"]
 OUT = os.path.join(HERE, "libdspb200.so")
 ARCH = ["-gencode", "arch=compute_90a,code=sm_90a"]
 

@@ -11,6 +11,7 @@
 #include "ops.h"
 #include "biquad_plan.h"
 #include "resample_plan.h"
+#include "io_plan.h"
 #include "fft.cuh"
 #include "../../include/dsp_b200.h"
 #include <cassert>
@@ -283,6 +284,8 @@ struct Shard {
 	std::vector<std::unique_ptr<Op>> ops;
 	double *buf[4] = { nullptr, nullptr, nullptr, nullptr };   // io-in, io-out/scratch, scratch, zeros
 	size_t cap = 0;   // doubles per buffer
+	void *stage = nullptr;   // host calls in another format than f64 interleaved: the caller's raw slab (io_plan.h)
+	size_t stage_cap = 0;    // bytes
 	static constexpr int DONE_RING = 8;
 	cudaEvent_t done[DONE_RING] = {};   // completion markers of submitted host blocks (ticket % DONE_RING)
 
@@ -291,6 +294,7 @@ struct Shard {
 		cudaSetDevice(device);
 		ops.clear();
 		for (double *b : buf) dev_free(b);
+		dev_free(stage);
 		for (cudaEvent_t e : done) if (e) cudaEventDestroy(e);
 		if (stream) cudaStreamDestroy(stream);
 	}
@@ -306,17 +310,27 @@ struct Shard {
 		return mx;
 	}
 
-	int ensure_cap(long frames)
+	// the working buffers for calls of `frames` frames, and the staging buffer of a host call in formats in_fmt / out_fmt
+	int ensure_cap(long frames, int in_fmt = IO_F64, int out_fmt = IO_F64)
 	{
-		const size_t need = (size_t) walk_max_frames(frames, nullptr) * ch_count;
-		if (need <= cap) return 0;
+		const long mx = walk_max_frames(frames, nullptr);
+		const size_t need = (size_t) mx * ch_count, stage_need = io_stage_bytes(in_fmt, out_fmt, ch_count, mx);
+		if (need <= cap && stage_need <= stage_cap) return 0;
 		CUDA_TRY(cudaStreamSynchronize(stream), return -1);
-		for (double *&b : buf) {
-			dev_free(b);
-			b = dev_alloc<double>(need, false);
-			if (!b) { cap = 0; return -1; }
+		if (need > cap) {
+			for (double *&b : buf) {
+				dev_free(b);
+				b = dev_alloc<double>(need, false);
+				if (!b) { cap = 0; return -1; }
+			}
+			cap = need;
 		}
-		cap = need;
+		if (stage_need > stage_cap) {
+			dev_free(stage);
+			stage = dev_alloc<char>(stage_need, false);
+			if (!stage) { stage_cap = 0; return -1; }
+			stage_cap = stage_need;
+		}
 		return 0;
 	}
 
@@ -370,6 +384,8 @@ struct Shard {
 }  // namespace dspb200
 
 using namespace dspb200;
+
+static_assert(DSPB200_IO_F64 == IO_F64 && DSPB200_IO_F32 == IO_F32 && DSPB200_IO_PLANAR == IO_PLANAR, "io_plan.h follows the ABI");
 
 struct dspb200_chain {
 	int fs = 0, channels = 0;
@@ -707,30 +723,45 @@ static void maybe_pin(dspb200_chain *c, const void *p, size_t bytes)
 	else cudaGetLastError();
 }
 
-static int copy_slab(const Shard &s, int C, long frames, double *dev, const double *host_in, double *host_out)
+// One H2D (host_in) or D2H (host_out) copy of `frames` frames of a shard's slab between the caller's buffer in format
+// `fmt` (planar rows `stride` elements apart) and the packed device slab `dev` (io_plan.h: io_copy).
+static int copy_slab(const Shard &s, int C, int fmt, long stride, long frames, void *dev, const void *host_in, void *host_out)
 {
-	const size_t w = (size_t) s.ch_count * sizeof(double), hp = (size_t) C * sizeof(double);
 	if (frames <= 0) return 0;
+	const IoCopy k = io_copy(fmt, stride, C, s.ch_begin, s.ch_count, frames);
 	(host_in ? g_h2d_copies : g_d2h_copies).fetch_add(1, std::memory_order_relaxed);
 	if (host_in) {
-		if (s.ch_count == C) CUDA_TRY(cudaMemcpyAsync(dev, host_in, w * frames, cudaMemcpyHostToDevice, s.stream), return -1);
-		else CUDA_TRY(cudaMemcpy2DAsync(dev, w, host_in + s.ch_begin, hp, w, frames, cudaMemcpyHostToDevice, s.stream), return -1);
+		const char *h = static_cast<const char *>(host_in) + k.host_off;
+		if (k.contiguous) CUDA_TRY(cudaMemcpyAsync(dev, h, k.width * k.height, cudaMemcpyHostToDevice, s.stream), return -1);
+		else CUDA_TRY(cudaMemcpy2DAsync(dev, k.dev_pitch, h, k.host_pitch, k.width, k.height, cudaMemcpyHostToDevice, s.stream), return -1);
 	}
 	else {
-		if (s.ch_count == C) CUDA_TRY(cudaMemcpyAsync(host_out, dev, w * frames, cudaMemcpyDeviceToHost, s.stream), return -1);
-		else CUDA_TRY(cudaMemcpy2DAsync(host_out + s.ch_begin, hp, dev, w, w, frames, cudaMemcpyDeviceToHost, s.stream), return -1);
+		char *h = static_cast<char *>(host_out) + k.host_off;
+		if (k.contiguous) CUDA_TRY(cudaMemcpyAsync(h, dev, k.width * k.height, cudaMemcpyDeviceToHost, s.stream), return -1);
+		else CUDA_TRY(cudaMemcpy2DAsync(h, k.host_pitch, dev, k.dev_pitch, k.width, k.height, cudaMemcpyDeviceToHost, s.stream), return -1);
 	}
 	return 0;
 }
 
-long dspb200_chain_submit_host(dspb200_chain *c, long frames, const double *in, double *out, unsigned long long *ticket)
+static bool io_refused(int in_fmt, long in_stride, int out_fmt, long out_stride, long frames, long max_out, bool same_buffer)
+{
+	char msg[256];
+	if (!io_check(in_fmt, in_stride, out_fmt, out_stride, frames, max_out, same_buffer, msg, sizeof(msg))) return false;
+	set_error("%s", msg);
+	return true;
+}
+
+long dspb200_chain_submit_host_io(dspb200_chain *c, long frames, const void *in, int in_fmt, long in_stride, void *out, int out_fmt,
+                                  long out_stride, unsigned long long *ticket)
 {
 	if (!c || !in || !out) return -1;
 	if (frames < 1) return 0;
 	const int C = c->channels;
 	const long max_out = dspb200_chain_max_out_frames(c, frames);
-	maybe_pin(c, in, (size_t) frames * C * sizeof(double));
-	if (out != in) maybe_pin(c, out, (size_t) ((max_out > frames) ? max_out : frames) * C * sizeof(double));
+	if (io_refused(in_fmt, in_stride, out_fmt, out_stride, frames, max_out, in == out)) return -1;
+	maybe_pin(c, in, io_host_bytes(in_fmt, in_stride, C, frames));
+	if (out != in) maybe_pin(c, out, io_host_bytes(out_fmt, out_stride, C, io_planar(out_fmt) ? max_out : (max_out > frames) ? max_out : frames));
+	const bool conv_in = io_kernel(in_fmt) >= 0, conv_out = io_kernel(out_fmt) >= 0;
 	long result = -1;
 	const unsigned long long t = c->ticket + 1;   // becomes current only when every shard has been enqueued
 	if (ticket && t > c->waited + Shard::DONE_RING) {
@@ -740,14 +771,23 @@ long dspb200_chain_submit_host(dspb200_chain *c, long frames, const double *in, 
 	}
 	FOR_EACH_SHARD(c, s) {
 		CUDA_TRY(cudaSetDevice(s->device), return -1);
-		if (s->ensure_cap(frames)) return -1;
-		if (copy_slab(*s, C, frames, s->buf[0], in, nullptr)) return -1;
+		if (s->ensure_cap(frames, in_fmt, out_fmt)) return -1;
+		// the staging buffer holds the caller's raw slab (a planar one with rows of `frames`, then `f` frames)
+		if (copy_slab(*s, C, in_fmt, in_stride, frames, conv_in ? s->stage : s->buf[0], in, nullptr)) return -1;
+		if (conv_in) {
+			edge_in(in_fmt, s->stage, frames, s->buf[0], s->ch_count, frames, s->stream);
+			if (take_launch_error()) return -1;
+		}
 		bool rate_change = false;
 		for (auto &op : s->ops) rate_change |= !op->inplace_ok;
 		double *dst = rate_change ? s->buf[3] : s->buf[0];
 		const long f = s->run_ops(0, frames, s->buf[0], dst, true, s->stream, /* one block at a time: */ ticket == nullptr);
 		if (f < 0) return -1;
-		if (copy_slab(*s, C, f, dst, nullptr, out)) return -1;
+		if (conv_out) {
+			edge_out(out_fmt, dst, s->stage, f, s->ch_count, f, s->stream);
+			if (take_launch_error()) return -1;
+		}
+		if (copy_slab(*s, C, out_fmt, out_stride, f, conv_out ? s->stage : dst, nullptr, out)) return -1;
 		if (ticket) {
 			cudaEvent_t &ev = s->done[t % Shard::DONE_RING];
 			if (!ev) CUDA_TRY(cudaEventCreateWithFlags(&ev, cudaEventDisableTiming), return -1);
@@ -758,6 +798,11 @@ long dspb200_chain_submit_host(dspb200_chain *c, long frames, const double *in, 
 	c->ticket = t;
 	if (ticket) *ticket = t;
 	return result;
+}
+
+long dspb200_chain_submit_host(dspb200_chain *c, long frames, const double *in, double *out, unsigned long long *ticket)
+{
+	return dspb200_chain_submit_host_io(c, frames, in, DSPB200_IO_F64, 0, out, DSPB200_IO_F64, 0, ticket);
 }
 
 int dspb200_chain_wait(dspb200_chain *c, unsigned long long ticket)
@@ -775,11 +820,12 @@ int dspb200_chain_wait(dspb200_chain *c, unsigned long long ticket)
 	return 0;
 }
 
-long dspb200_chain_run_host(dspb200_chain *c, long frames, const double *in, double *out)
+long dspb200_chain_run_host_io(dspb200_chain *c, long frames, const void *in, int in_fmt, long in_stride, void *out, int out_fmt,
+                               long out_stride)
 {
 	if (!c || !in || !out) return -1;
 	if (frames < 1) return 0;
-	const long result = dspb200_chain_submit_host(c, frames, in, out, nullptr);
+	const long result = dspb200_chain_submit_host_io(c, frames, in, in_fmt, in_stride, out, out_fmt, out_stride, nullptr);
 	// also after a failed submit: nothing of this call may still be in flight when we return
 	FOR_EACH_SHARD(c, s) {
 		cudaSetDevice(s->device);
@@ -789,7 +835,13 @@ long dspb200_chain_run_host(dspb200_chain *c, long frames, const double *in, dou
 	return result;
 }
 
-long dspb200_chain_run_device(dspb200_chain *c, int shard, long frames, const double *d_in, double *d_out, void *stream)
+long dspb200_chain_run_host(dspb200_chain *c, long frames, const double *in, double *out)
+{
+	return dspb200_chain_run_host_io(c, frames, in, DSPB200_IO_F64, 0, out, DSPB200_IO_F64, 0);
+}
+
+long dspb200_chain_run_device_io(dspb200_chain *c, int shard, long frames, const void *d_in, int in_fmt, long in_stride, void *d_out,
+                                 int out_fmt, long out_stride, void *stream)
 {
 	if (!c || shard < 0 || shard >= (int) c->shards.size() || !d_in || !d_out) return -1;
 	if (frames < 1) return 0;
@@ -800,10 +852,41 @@ long dspb200_chain_run_device(dspb200_chain *c, int shard, long frames, const do
 		set_error("chain: in-place call on a chain whose last operator changes the frame count");
 		return -1;
 	}
+	long max_out = frames;
+	s->walk_max_frames(frames, &max_out);
+	if (io_refused(in_fmt, in_stride, out_fmt, out_stride, frames, max_out, d_in == d_out)) return -1;
+	if (!io_aligned((uintptr_t) d_in, in_fmt) || !io_aligned((uintptr_t) d_out, out_fmt)) {
+		set_error("io: a device buffer is not aligned to its element type (%zu bytes in, %zu out)", io_esize(in_fmt), io_esize(out_fmt));
+		return -1;
+	}
 	CUDA_TRY(cudaSetDevice(s->device), return -1);
 	if (s->ensure_cap(frames)) return -1;
 	cudaStream_t st = (cudaStream_t) stream;   // NULL = the legacy default stream, as everywhere in CUDA
-	return s->run_ops(0, frames, d_in, d_out, false, st, false);
+	const bool conv_in = io_kernel(in_fmt) >= 0, conv_out = io_kernel(out_fmt) >= 0;
+	if (!conv_in && !conv_out) return s->run_ops(0, frames, (const double *) d_in, (double *) d_out, false, st, false);
+	// the edge kernels read d_in and write d_out directly; the operators run on the shard's own buffers in between
+	// (buf[0] holds the converted input, and is the result when no operator changes the frame count)
+	const double *src = (const double *) d_in;
+	if (conv_in) {
+		edge_in(in_fmt, d_in, in_stride, s->buf[0], s->ch_count, frames, st);
+		if (take_launch_error()) return -1;
+		src = s->buf[0];
+	}
+	bool rate_change = false;
+	for (auto &op : s->ops) rate_change |= !op->inplace_ok;
+	double *dst = !conv_out ? (double *) d_out : (conv_in && rate_change) ? s->buf[3] : s->buf[0];
+	const long f = s->run_ops(0, frames, src, dst, conv_in, st, false);
+	if (f < 0) return -1;
+	if (conv_out) {
+		edge_out(out_fmt, dst, d_out, out_stride, s->ch_count, f, st);
+		if (take_launch_error()) return -1;
+	}
+	return f;
+}
+
+long dspb200_chain_run_device(dspb200_chain *c, int shard, long frames, const double *d_in, double *d_out, void *stream)
+{
+	return dspb200_chain_run_device_io(c, shard, frames, d_in, DSPB200_IO_F64, 0, d_out, DSPB200_IO_F64, 0, stream);
 }
 
 int dspb200_chain_join(dspb200_chain *c, int shard, void *stream)
@@ -825,15 +908,17 @@ int dspb200_debug_read(dspb200_chain *c, int shard, int op_index, long long *out
 	return s->ops[op_index]->debug_read(out, max);
 }
 
-long dspb200_chain_drain_host(dspb200_chain *c, long frames, double *out)
+long dspb200_chain_drain_host_io(dspb200_chain *c, long frames, void *out, int out_fmt, long out_stride)
 {
 	// the drain2 half of drain_effects_chain(), effects_chain.c:1199-1217
 	if (!c || !out || frames < 1) return -1;
 	const int C = c->channels;
+	if (io_refused(IO_F64, 0, out_fmt, out_stride, frames, dspb200_chain_max_out_frames(c, frames), false)) return -2;
+	const bool conv_out = io_kernel(out_fmt) >= 0;
 	long result = -1;
 	FOR_EACH_SHARD(c, s) {
 		CUDA_TRY(cudaSetDevice(s->device), return -2);
-		if (s->ensure_cap(frames)) return -2;
+		if (s->ensure_cap(frames, IO_F64, out_fmt)) return -2;
 		long ftmp = frames, dframes = -1;
 		size_t idx = 0;
 		double *cur = s->buf[0];
@@ -850,7 +935,11 @@ long dspb200_chain_drain_host(dspb200_chain *c, long frames, double *out)
 		double *dst = s->buf[3];   // the silence buffer is free again once drain2 has run
 		const long f = s->run_ops(idx, dframes, cur, dst, true, s->stream);
 		if (f < 0) return -2;
-		if (copy_slab(*s, C, f, dst, nullptr, out)) return -2;
+		if (conv_out) {
+			edge_out(out_fmt, dst, s->stage, f, s->ch_count, f, s->stream);
+			if (take_launch_error()) return -2;
+		}
+		if (copy_slab(*s, C, out_fmt, out_stride, f, conv_out ? s->stage : dst, nullptr, out)) return -2;
 		result = f;
 	}
 	FOR_EACH_SHARD(c, s) {
@@ -858,6 +947,11 @@ long dspb200_chain_drain_host(dspb200_chain *c, long frames, double *out)
 		CUDA_TRY(cudaStreamSynchronize(s->stream), return -2);
 	}
 	return result;
+}
+
+long dspb200_chain_drain_host(dspb200_chain *c, long frames, double *out)
+{
+	return dspb200_chain_drain_host_io(c, frames, out, DSPB200_IO_F64, 0);
 }
 
 void dspb200_chain_reset(dspb200_chain *c)

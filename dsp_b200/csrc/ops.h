@@ -24,6 +24,11 @@ Op *make_resample_op(int slab_channels, int fs_in, int fs_out, double bandwidth,
 struct ResampleParams;
 int resample_params_or_error(int fs_in, int fs_out, double bw, ResampleParams *p);
 
+// edge.cu: a block in the caller's format (io_plan.h; planar rows `stride` elements apart) <-> the working buffer, C
+// channels of interleaved doubles; nothing is launched for f64 interleaved
+void edge_in(int fmt, const void *src, long stride, double *dst, int C, long frames, cudaStream_t st);
+void edge_out(int fmt, const double *src, void *dst, long stride, int C, long frames, cudaStream_t st);
+
 void fir_debug_serialize(int on);
 int fir_debug_stall(int roles, int us, int period, int phase);
 int test_rfft(int B, int n_ch, const double *d_in, double *d_spec, cudaStream_t st);

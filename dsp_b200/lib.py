@@ -2,7 +2,8 @@
 
 There is no CPU path: if the CUDA library is missing or no device is usable, constructing a
 Chain raises.  numpy arrays are host buffers (mode A); raw device pointers + a cudaStream_t
-(e.g. from torch tensors / torch.cuda.current_stream().cuda_stream) are mode D.
+(e.g. from torch tensors / torch.cuda.current_stream().cuda_stream) are mode D.  Chain.run_io and Chain.run_tensor
+take float32 or float64 blocks, interleaved [frames, channels] or planar [channels, frames] (the _io calls).
 """
 import ctypes as C
 import os
@@ -56,6 +57,12 @@ SIGNATURES = {
     "dspb200_chain_sync": (C.c_int, [C.c_void_p]),
     "dspb200_chain_submit_host": (C.c_long, [C.c_void_p, C.c_long, C.c_void_p, C.c_void_p, C.POINTER(C.c_ulonglong)]),
     "dspb200_chain_wait": (C.c_int, [C.c_void_p, C.c_ulonglong]),
+    "dspb200_chain_run_host_io": (C.c_long, [C.c_void_p, C.c_long, C.c_void_p, C.c_int, C.c_long, C.c_void_p, C.c_int, C.c_long]),
+    "dspb200_chain_submit_host_io": (C.c_long, [C.c_void_p, C.c_long, C.c_void_p, C.c_int, C.c_long, C.c_void_p, C.c_int, C.c_long,
+                                                C.POINTER(C.c_ulonglong)]),
+    "dspb200_chain_run_device_io": (C.c_long, [C.c_void_p, C.c_int, C.c_long, C.c_void_p, C.c_int, C.c_long, C.c_void_p, C.c_int,
+                                               C.c_long, C.c_void_p]),
+    "dspb200_chain_drain_host_io": (C.c_long, [C.c_void_p, C.c_long, C.c_void_p, C.c_int, C.c_long]),
     "dspb200_biquad_design": (C.c_int, [C.c_int, C.c_double, C.c_double, C.c_double, C.c_double, C.c_double, C.c_int, _dp]),
     "dspb200_hilbert_taps": (C.c_int, [C.c_long, C.c_double, _dp]),
     "dspb200_resample_params": (C.c_int, [C.c_int, C.c_int, C.c_double, _lp]),
@@ -66,6 +73,28 @@ SIGNATURES = {
 
 class DspB200Error(RuntimeError):
     pass
+
+
+# sample formats of the _io calls (DSPB200_IO_* in include/dsp_b200.h): a type | a layout
+IO_F64, IO_F32, IO_PLANAR = 0, 1, 0x10
+
+
+def io_format(dtype, planar):
+    """The DSPB200_IO_* format of samples of `dtype` (float32 or float64) in the given layout."""
+    dtype = np.dtype(dtype)
+    if dtype not in (np.float32, np.float64):
+        raise DspB200Error("sample formats are float32 and float64, not %s" % dtype)
+    return (IO_F32 if dtype == np.float32 else IO_F64) | (IO_PLANAR if planar else 0)
+
+
+def _io_stride(shape, strides, itemsize, planar):
+    """(rows stride in elements for the ABI, True when the array's layout needs no copy) of a 2-D array."""
+    if planar:
+        ok = shape[1] <= 1 or strides[1] == itemsize
+        ok = ok and strides[0] % itemsize == 0 and strides[0] >= 0 and (shape[0] <= 1 or strides[0] // itemsize >= shape[1])
+        return (strides[0] // itemsize if shape[0] > 1 else shape[1]), ok
+    ok = (shape[1] <= 1 or strides[1] == itemsize) and (shape[0] <= 1 or strides[0] == shape[1] * itemsize)
+    return 0, ok
 
 
 def lib():
@@ -260,6 +289,85 @@ class Chain:
     def wait(self, ticket):
         _check(lib().dspb200_chain_wait(self.h, int(ticket)), "wait")
 
+    def run_io(self, x, planar=False, out=None):
+        """Mode A in the caller's format: x a float32 or float64 host array, [frames, channels] or, planar,
+        [channels, frames] (rows may be further apart than `frames`).  Returns `out` (or a new array of x's dtype) cut to
+        the returned frames, in the same layout.  out may be wider than the result; its dtype sets the output format."""
+        x = np.asarray(x)
+        if x.ndim != 2 or x.shape[0 if planar else 1] != self.channels:
+            raise DspB200Error("run_io: expected %s, got shape %s" % ("[channels, frames]" if planar else "[frames, channels]", x.shape))
+        in_fmt = io_format(x.dtype, planar)
+        in_stride, ok = _io_stride(x.shape, x.strides, x.itemsize, planar)
+        if not ok:
+            x = np.ascontiguousarray(x)
+            in_stride, _ = _io_stride(x.shape, x.strides, x.itemsize, planar)
+        frames = x.shape[1 if planar else 0]
+        n_out = max(self.max_out_frames(frames), frames if not planar else 0, 1)
+        if out is None:
+            out = np.empty((self.channels, n_out) if planar else (n_out, self.channels), dtype=x.dtype)
+        out_fmt = io_format(out.dtype, planar)
+        out_stride, ok = _io_stride(out.shape, out.strides, out.itemsize, planar)
+        if not ok or out.shape[0 if planar else 1] != self.channels:
+            raise DspB200Error("run_io: out must be a writable %s array with unit-stride rows" % ("[channels, W]" if planar else "[frames, channels]"))
+        n = _check(lib().dspb200_chain_run_host_io(self.h, frames, x.ctypes.data, in_fmt, in_stride, out.ctypes.data, out_fmt, out_stride),
+                   "run_host_io")
+        return out[:, :n] if planar else out[:n]
+
+    def run_io_raw(self, frames, in_ptr, in_fmt, in_stride, out_ptr, out_fmt, out_stride):
+        """run_raw in the caller's formats (IO_* | IO_PLANAR); strides in elements, 0 for interleaved buffers."""
+        return _check(lib().dspb200_chain_run_host_io(self.h, int(frames), in_ptr, int(in_fmt), int(in_stride), out_ptr, int(out_fmt),
+                                                      int(out_stride)), "run_host_io")
+
+    def submit_io_raw(self, frames, in_ptr, in_fmt, in_stride, out_ptr, out_fmt, out_stride):
+        """submit_raw in the caller's formats: returns (out_frames, ticket); buffers stay busy until wait(ticket)."""
+        t = C.c_ulonglong(0)
+        n = _check(lib().dspb200_chain_submit_host_io(self.h, int(frames), in_ptr, int(in_fmt), int(in_stride), out_ptr, int(out_fmt),
+                                                      int(out_stride), C.byref(t)), "submit_host_io")
+        return n, t.value
+
+    def run_device_io(self, shard, frames, d_in, in_fmt, in_stride, d_out, out_fmt, out_stride, stream=None):
+        """run_device in the caller's formats (raw device pointers, strides in elements)."""
+        return _check(lib().dspb200_chain_run_device_io(self.h, int(shard), int(frames), d_in, int(in_fmt), int(in_stride), d_out,
+                                                        int(out_fmt), int(out_stride), stream), "run_device_io")
+
+    def run_tensor(self, x, planar=True, out=None):
+        """Mode D on torch.cuda.current_stream(): x a CUDA tensor, float32 or float64, [channels, T] (planar, the
+        default) or [T, channels].  Returns `out` (or a new tensor of x's dtype) cut to the returned frames, in the same
+        layout; out may be wider than the result and in place (out is x) where the chain allows it.  Single-shard
+        chains only."""
+        import torch
+        if self.n_shards != 1:
+            raise DspB200Error("run_tensor: the chain has %d shards; run_tensor drives single-shard chains (use run_device_io per shard)"
+                               % self.n_shards)
+        if not (isinstance(x, torch.Tensor) and x.is_cuda and x.dim() == 2):
+            raise DspB200Error("run_tensor: expected a 2-D CUDA tensor")
+        if x.shape[0 if planar else 1] != self.channels:
+            raise DspB200Error("run_tensor: expected %s with %d channels, got %s" % ("[channels, T]" if planar else "[T, channels]",
+                                                                                    self.channels, tuple(x.shape)))
+        dev = self.shard_info(0)[0]
+        if x.device.index != dev:
+            raise DspB200Error("run_tensor: the chain runs on cuda:%d, x is on %s" % (dev, x.device))
+        isz = x.element_size()
+        in_fmt = io_format(str(x.dtype).replace("torch.", ""), planar)
+        in_stride, ok = _io_stride(tuple(x.shape), tuple(s * isz for s in x.stride()), isz, planar)
+        if not ok:
+            x = x.contiguous()
+            in_stride, _ = _io_stride(tuple(x.shape), tuple(s * isz for s in x.stride()), isz, planar)
+        frames = x.shape[1 if planar else 0]
+        n_out = max(self.max_out_frames(frames), 1)
+        if out is None:
+            out = torch.empty((self.channels, n_out) if planar else (n_out, self.channels), dtype=x.dtype, device=x.device)
+        osz = out.element_size()
+        out_fmt = io_format(str(out.dtype).replace("torch.", ""), planar)
+        out_stride, ok = _io_stride(tuple(out.shape), tuple(s * osz for s in out.stride()), osz, planar)
+        if not ok or out.device != x.device or out.shape[0 if planar else 1] != self.channels:
+            raise DspB200Error("run_tensor: out must be a %s tensor on %s with unit-stride rows" % ("[channels, W]" if planar else "[T, channels]",
+                                                                                                  x.device))
+        with torch.cuda.device(x.device):
+            stream = torch.cuda.current_stream().cuda_stream
+        n = self.run_device_io(0, frames, x.data_ptr(), in_fmt, in_stride, out.data_ptr(), out_fmt, out_stride, stream)
+        return out[:, :n] if planar else out[:n]
+
     def run_device(self, shard, frames, d_in, d_out, stream=None):
         """Mode D: raw device pointers (ints), asynchronous on `stream` (cudaStream_t as int)."""
         return _check(lib().dspb200_chain_run_device(self.h, int(shard), int(frames), d_in, d_out, stream), "run_device")
@@ -283,6 +391,19 @@ class Chain:
         if n < 0:
             raise DspB200Error("drain_host failed: " + last_error())
         return out[:n].copy()
+
+    def drain_io(self, frames, dtype=np.float64, planar=False):
+        """drain() in the caller's format: a [frames, channels] or, planar, [channels, frames] array of `dtype`; None when
+        dry."""
+        n_out = max(self.max_out_frames(frames), 1)
+        out = np.empty((self.channels, n_out) if planar else (n_out, self.channels), dtype=dtype)
+        fmt = io_format(dtype, planar)
+        n = lib().dspb200_chain_drain_host_io(self.h, int(frames), out.ctypes.data, fmt, n_out if planar else 0)
+        if n == -1:
+            return None
+        if n < 0:
+            raise DspB200Error("drain_host_io failed: " + last_error())
+        return (out[:, :n] if planar else out[:n]).copy()
 
     def process(self, x, block, drain_frames=0):
         """Whole stream in `block`-frame calls, then `drain_frames` of silence (the chain's

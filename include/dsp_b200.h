@@ -51,7 +51,7 @@ long long dspb200_kernel_launches(void);
 
 /* Per-kernel device timing for bench.py's roofline line: while enabled, the hot kernels are
  * bracketed by CUDA events on the stream they are launched on.  `name` is one of
- * "fir_mac", "fir_fwd", "fir_inv", "biquad", "resample"; read() waits for the events, returns
+ * "fir_mac", "fir_fwd", "fir_inv", "biquad", "resample", "edge" (the sample-format conversions); read() waits for the events, returns
  * the summed milliseconds and the launch count since the last read, and clears them. */
 void dspb200_profile_enable(int on);
 int  dspb200_profile_read(const char *name, double *total_ms, long *launches);
@@ -164,6 +164,36 @@ int  dspb200_debug_read(dspb200_chain *c, int shard, int op_index, long long *ou
  * until every rate-changing operator is dry.  Returns frames written (0..max_frames*ratio),
  * or -1 when nothing is left. */
 long dspb200_chain_drain_host(dspb200_chain *c, long frames, double *out);
+
+/* ---- sample formats at the edge -------------------------------------------------------- */
+/* The _io variants of the four block calls take the caller's buffers in any of four formats, chosen independently
+ * for input and output: a sample type | a layout.
+ *   DSPB200_IO_F64 / DSPB200_IO_F32: IEEE double / float samples.
+ *   interleaved (no layout bit): buf[frame * channels + channel], as everywhere else here; the stride is 0.
+ *   DSPB200_IO_PLANAR: channel k's row starts at base + k * stride elements (numpy / torch [channels, frames]);
+ *     stride >= frames on input, and >= dspb200_chain_max_out_frames(c, frames) on output.
+ * Inside, every shard works on interleaved doubles as always; the conversion is one pass over the block on the
+ * device (edge.cu), after the copy in and before the copy out.  It carries no policy: float -> double is exact,
+ * double -> float rounds to nearest even with subnormals kept, values beyond FLT_MAX become +-Inf, and +-0, +-Inf
+ * and NaN pass through (NaN payloads may be canonicalised).  f64 interleaved through an _io call is exactly the
+ * plain call: no extra kernel, no staging copy.
+ * Refusals: unknown format bits, a non-zero stride on an interleaved buffer, a short planar stride, and in == out with
+ * a different format or stride on the two sides; each returns < 0 (-2 from drain_host_io) with a message in
+ * dspb200_last_error() before anything is enqueued, and leaves the chain's state as it was.  Of the output only the
+ * returned frames of each row are written; padding between planar rows is never touched.
+ * Host calls: one host->device and one device->host copy per shard and call in every format (a planar shard's
+ * channel slab is a run of consecutive rows: one 2-D copy); page-locking (DSP_B200_PIN) and the ticket ring work on
+ * the caller's byte sizes.  Mode D: the buffers hold the shard's slab (a planar caller passes the address of the
+ * slab's first row) and need only the alignment of their element type; the stream-ordering and "d_in is never
+ * written unless in place" guarantees of dspb200_chain_run_device hold, as does its in-place rule. */
+enum { DSPB200_IO_F64 = 0, DSPB200_IO_F32 = 1, DSPB200_IO_PLANAR = 0x10 };
+long dspb200_chain_run_host_io(dspb200_chain *c, long frames, const void *in, int in_fmt, long in_stride,
+                               void *out, int out_fmt, long out_stride);
+long dspb200_chain_submit_host_io(dspb200_chain *c, long frames, const void *in, int in_fmt, long in_stride,
+                                  void *out, int out_fmt, long out_stride, unsigned long long *ticket);
+long dspb200_chain_run_device_io(dspb200_chain *c, int shard, long frames, const void *d_in, int in_fmt, long in_stride,
+                                 void *d_out, int out_fmt, long out_stride, void *stream);
+long dspb200_chain_drain_host_io(dspb200_chain *c, long frames, void *out, int out_fmt, long out_stride);
 
 void dspb200_chain_reset(dspb200_chain *c);     /* effect->reset() of every operator */
 int  dspb200_chain_sync(dspb200_chain *c);      /* wait for all shards' streams */
